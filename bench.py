@@ -47,7 +47,9 @@ def parse_args():
                     help="frames per kb_integrate_frames call; 0 (default) = the whole step in one call (the library fuses 32 frames "
                          "per kernel group inside a call and pipelines the groups); 1 = per-frame calls")
     ap.add_argument("--lap-frames", type=int, default=5000, help="frames in one lap of the trajectory (pool in HBM)")
-    ap.add_argument("--max-blocks", type=int, default=90000)
+    ap.add_argument("--max-blocks", type=int, default=45000,
+                    help="block pool per map (the hall640 lap allocates ~25.6 k blocks; the dynamic leg holds a second map, "
+                         "and both must fit beside the lap in 80 GB)")
     ap.add_argument("--cpu-sample-frames", type=int, default=5000,
                     help="upper bound on the frames of the cpu_baseline sample (it stops after --cpu-sample-seconds)")
     ap.add_argument("--cpu-sample-seconds", type=float, default=12.0, help="CPU work of the cpu_baseline sample")
@@ -93,6 +95,10 @@ def parse_args():
                     help="N > 1: resident fusion CTAs per SM (KB_FUSE_CTAS_PER_SM; 0 = library default = full occupancy). Fewer CTAs leave "
                          "registers for the next batch's block selection / culling kernels to run beside the fusion kernel")
     ap.add_argument("--small", action="store_true", help="tiny configuration for functional checks")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the map they produced as DIR/<name>.npy (single GPU, hall workloads): "
+                         "the map checksum, every block index and a seeded sample of blocks' voxels, so that two builds "
+                         "can be compared output for output")
     ap.add_argument("--workload", default="hall640", choices=["hall640", "hall1280", "dynamic"],
                     help="hall640 = BASELINE config[1] (fusion only, the headline, used for every --gpus N); hall1280 = "
                          "config[3] shapes (1280x720, 2 cm voxels: ~20x the voxel work per frame) for the sharded "
@@ -125,7 +131,7 @@ def algorithmic_bytes(nv, nsem, nblk, pixels, lp=20, bpp=BYTES_PER_PIXEL_IN):
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md). The timed region of the
+    """Samples nvidia-smi clocks/throttle reasons during the timed region. The timed region of the
     default run is ~0.1 s, so nvidia-smi is started early (before the last warm-up step: its start-up latency is of
     that order) with a 20 ms period, every sample is stamped on arrival, and stop(t0, t1) keeps the samples that fell
     inside the timed window [t0, t1] (perf_counter seconds)."""
@@ -191,7 +197,9 @@ def map_configs(args):
     mb = args.max_blocks if not args.small else 8192
     msem = 0
     if args.workload == "hall1280" and not args.small:
-        mb = max(args.max_blocks, 420000) // world + 20000   # block-hash shard: 1/N of the map per GPU
+        # block-hash shard: 1/N of the map per GPU. The hall allocates ~74 k blocks; 120 k blocks + 60 k semantic
+        # blocks take ~29 GB, which leaves room for the lap of frames on one 80 GB GPU
+        mb = max(args.max_blocks, 100000) // world + 20000
         msem = mb // 2
     mc = capi.default_map_config(voxel_size=vs, vps=16, trunc=tr, with_semantics=True, with_tracking=True,
                                  max_blocks=mb, max_semantic_blocks=msem)
@@ -500,21 +508,8 @@ def emit(obj):
     print(json.dumps(obj), flush=True)
 
 
-def load_capture():
-    """Per-launch DRAM traffic / issue utilisation of the dominant kernel from THIS round's `ncu --set full` capture
-    (profiles/r2_fuse_capture.json, written by tools/ncu_digest.py from the committed csv export). None if absent."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "r2_fuse_capture.json")))
-    except Exception:
-        return None
-
-
 def hbm_peak():
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        return float(peaks["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (of measured)"
-    except Exception:
-        return 6650.0, "fallback 6650 (of fallback)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
 GROUP = 32  # frames fused per kernel group inside a kb_integrate_frames call (csrc/kb_kernels.cuh kMaxBatch)
@@ -534,21 +529,12 @@ def roofline_block(args, B, n_calls, gpu_ms, sampled_us, nv, nsem, nblk, n_frame
     per_launch = total_bytes / max(n_calls, 1)
     avg_us = gpu_ms * 1e3 / max(n_calls, 1)
     achieved = total_bytes / (gpu_ms * 1e-3) / 1e9
-    cap = load_capture()
-    traffic = issue = None
-    if cap and cap.get("frames_per_launch") == B and args.workload == "hall640" and not args.small and world == 1:
-        traffic = cap.get("dram_bytes_per_launch_group")
-        issue = cap.get("fuse_issue_slot_utilization_pct")
-    out = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+    out = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
            "kernel": "fuseKernel<16> + its prologue (tileMax, tilePyramid, selectBlocks, itemCull, itemCompact): one group per %d frames" % B,
            "launch_us": avg_us, "launch_us_sampled": sampled_us, "algorithmic_bytes_per_launch": per_launch,
            "peak_source": src,
-           "note": "the kernel is issue-bound, not HBM-bound (DRAM traffic is below the algorithmic bytes: the working set is L2 "
-                   "resident); frac_dram = measured DRAM bytes / time / peak, issue_slot_utilization from the same ncu capture"}
-    if traffic:
-        out["frac_dram"] = traffic / (avg_us * 1e-6) / 1e9 / peak
-    if issue is not None:
-        out["issue_slot_utilization_pct"] = issue
+           "note": "algorithmic bytes, not measured DRAM traffic: the per-batch working set is largely L2 resident, so the "
+                   "kernel is expected to be issue-bound rather than HBM-bound"}
     return out
 
 
@@ -595,7 +581,7 @@ def main_hall_cells(args, world, rank, local_rank, dev):
     gx, gy = rank_grid(world)
     # which ranks need which frame: pure pose arithmetic (kb_frame_owners), identical on every rank. The per-batch cost of a
     # rank is dominated by fixed work per frame it receives (tile pyramid, block selection, the critical path of the fusion
-    # kernel), so the layout with the fewest frames on the busiest rank wins (measured: profiles/r2_multigpu_summary.txt).
+    # kernel), so the layout with the fewest frames on the busiest rank wins.
     probe_frames = [h.make_frame(None, poses[g], stamps[g]) for g in range(lap)]
     frames_of = lambda m_: [int(((m_ >> r) & 1).sum()) for r in range(world)]
     layouts = {}
@@ -852,7 +838,7 @@ def main_hall_cells(args, world, rank, local_rank, dev):
             "exchange": {"kind": "one-sided NVLink pull (kb_gather_run), overlapped with the previous step's fusion",
                          "bytes_pulled_all_ranks": float(A[:, 6].sum()), "gbps_per_rank": [round(x, 1) for x in gbps],
                          "gather_ms_per_rank": [round(float(x), 2) for x in A[:, 5]],
-                         "reference_gbps": 770.0, "reference": "measured peer copy per direction (B200_PROFILING.md)"},
+                         "reference_gbps": 450.0, "reference": "H100 SXM NVLink 4 data sheet, per direction (not measured)"},
             "checksum": combine_checksums(parts),
             "roofline": roof, "cpu_baseline": None, "e2e": e2e, "gpu_launches": 6 * n_calls, "clocks": clocks, "wall_s_timed": wall,
         }
@@ -867,9 +853,40 @@ def main_hall_cells(args, world, rank, local_rank, dev):
     return None
 
 
+DUMP_SAMPLE_BLOCKS = 256  # 24 MB of voxel fields; the full map is ~2 GB without likelihoods
+
+
+def dump_outputs(h, cs, out_dir):
+    """Writes the map after the timed steps: the checksum over every voxel (u64 words split into exact 32-bit halves),
+    every block index, and distance / weight / semantic label / last_observed of a seeded sample of blocks. Blocks are
+    exported sorted by index, so the sample is the same for every build that computes the same map."""
+    from khronos_b200 import capi
+    n, V = h.num_blocks(), h.V
+    bi = np.zeros((n, 3), np.int32)
+    dist, wgt = np.zeros((n, V), np.float32), np.zeros((n, V), np.float32)
+    lab, obs = np.zeros((n, V), np.uint32), np.zeros((n, V), np.uint64)
+    ex = capi.BlockExport(block_index=bi.ctypes.data, distance=dist.ctypes.data, weight=wgt.ctypes.data,
+                          semantic_label=lab.ctypes.data, last_observed=obs.ctypes.data)
+    nw = ctypes.c_int32(0)
+    h._check(h._fn("export_blocks")(h._h, capi.EXPORT_ALL, n, ctypes.byref(ex), ctypes.byref(nw)))
+    if nw.value != n:
+        raise RuntimeError(f"kb_export_blocks wrote {nw.value} of {n} blocks")
+    words = [int(c) for c in cs]
+    halves = [w >> s & 0xFFFFFFFF for w in words[:2] for s in (32, 0)]
+    sel = np.sort(np.random.default_rng(0).choice(n, size=min(DUMP_SAMPLE_BLOCKS, n), replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"map_checksum": np.array(halves + words[2:], np.float64), "block_index": bi.astype(np.float64),
+              "sample_block_index": bi[sel].astype(np.float64), "sample_distance": dist[sel], "sample_weight": wgt[sel],
+              "sample_semantic_label": lab[sel].astype(np.float64), "sample_last_observed_ns": obs[sel].astype(np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def main():
     args = parse_args()
     quiet_stdout()
+    if args.dump_outputs and (args.impl == "reference" or args.workload == "dynamic" or int(os.environ.get("WORLD_SIZE", "1")) > 1):
+        raise SystemExit("--dump-outputs: only the single-GPU hall workloads write their outputs")
     if args.impl == "reference":
         return main_reference(args)
     if args.workload == "dynamic":
@@ -1101,6 +1118,8 @@ def main():
         raise SystemExit("bench.py: block pool exhausted (capacity_exceeded): results incomplete")
     # order-independent checksum of the map after the timed region (same value for every --gpus N: the bench verifies itself)
     cs = h.map_checksum()
+    if args.dump_outputs:
+        dump_outputs(h, cs, args.dump_outputs)
     pairs = t64_1.block_frame_pairs - t64_0.block_frame_pairs
     n_frames = K * F
     # 64-bit cumulative counters (kb_get_totals64): the 32-bit ones wrap after ~36 k frames of this workload

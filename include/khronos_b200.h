@@ -1,5 +1,5 @@
 /*
- * khronos_b200.h — C ABI of the B200-native active-window volumetric integrator.
+ * khronos_b200.h — C ABI of the H100-native active-window volumetric integrator.
  *
  * This is the drop-in boundary for Khronos' per-frame active-window fusion hot path. Every entry
  * point cites the reference interface it replaces (paths relative to the Khronos checkout;

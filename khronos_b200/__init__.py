@@ -1,4 +1,4 @@
-"""khronos_b200 — B200-native active-window volumetric integrator for Khronos.
+"""khronos_b200 — H100-native active-window volumetric integrator for Khronos.
 
 The product is the CUDA library ``khronos_b200/csrc/libkhronos_b200.so`` behind the C ABI of
 ``include/khronos_b200.h``; this package is the thin Python host mirror used by tests and bench.

@@ -1,4 +1,4 @@
-"""Builds the in-tree CUDA product library (sm_100a) and, for tests, the CPU oracle."""
+"""Builds the in-tree CUDA product library (sm_90a, H100) and, for tests, the CPU oracle."""
 from __future__ import annotations
 
 import os
@@ -13,7 +13,7 @@ HEADERS = ["kb_device.cuh", "kb_kernels.cuh", "kb_motion_device.cuh", "kb_object
 LIB = os.path.join(CSRC, "libkhronos_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     # bit-parity with the fp32 reference arithmetic: no FMA contraction on device or host
     "-fmad=false", "-Xcompiler", "-fPIC,-ffp-contract=off,-fno-fast-math", "-shared",
 ]

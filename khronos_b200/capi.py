@@ -637,7 +637,7 @@ def load_product_library() -> C.CDLL:
     if not os.path.exists(path):
         raise ImportError(
             f"{path} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). khronos_b200 has no CPU fallback.")
+            "(nvcc, sm_90a). khronos_b200 has no CPU fallback.")
     return C.CDLL(path, mode=C.RTLD_GLOBAL)
 
 

@@ -1,4 +1,4 @@
-// C ABI (include/khronos_b200.h) over the sm_100a kernels: handle lifetime, device memory, frame
+// C ABI (include/khronos_b200.h) over the sm_90a kernels: handle lifetime, device memory, frame
 // staging, stamp <-> frame-index bookkeeping, export. Host code only; no CPU compute fallback exists:
 // every entry point that touches voxels launches a kernel, and kb_create refuses to run without a GPU.
 #include <algorithm>
@@ -65,10 +65,10 @@ struct kb_handle {
   uint32_t* item_fmask = nullptr;
   int* item_list = nullptr;    // KB_FUSE_ITEM_LIST experiment: compacted heaviest-first item lists (3 x item_list_cap)
   int item_list_cap = 0;
-  bool use_item_list = true;   // default since round 2 (+7 % alone, +40 % with the pipeline; profiles/r2_ab1_summary.txt); KB_FUSE_ITEM_LIST=0 disables
+  bool use_item_list = true;   // default since round 2 (won its A/B); KB_FUSE_ITEM_LIST=0 disables
   // KB_PIPELINE experiment: the prologue (tile pyramid, K0, K0b[, compaction]) of batch i+1 runs on its own stream while
   // the fuse kernel of batch i is still busy; work lists, tile pyramids and cursors exist twice (index = batch parity)
-  bool pipelined = true;       // default since round 2 (+31 %, profiles/r2_ab1_summary.txt); KB_PIPELINE=0 disables
+  bool pipelined = true;       // default since round 2 (won its A/B); KB_PIPELINE=0 disables
   cudaStream_t pre_stream = nullptr;
   cudaEvent_t pre_done[2] = {nullptr, nullptr}, fuse_done[2] = {nullptr, nullptr}, main_front = nullptr;
   bool main_dirty = true;      // main-stream work other than fuse kernels was enqueued since the last prologue

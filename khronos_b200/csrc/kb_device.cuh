@@ -1,4 +1,4 @@
-// Device-side data layout and helpers of the B200 volumetric map (sm_100a).
+// Device-side data layout and helpers of the volumetric map (sm_90a).
 //
 // HBM layout (all arrays are structure-of-arrays over a fixed pool of block slots, V = vps^3):
 //   hash_keys[H] u64, hash_vals[H] i32      open-addressed block hash (linear probing, tombstones)
@@ -264,5 +264,14 @@ __device__ __forceinline__ void evalTracking(const DeviceMap& m, const TrackEval
   *to_remove = rem;
 }
 #endif
+
+// Streaming multiprocessors of the current device (132 on an H100 SXM): the grid unit of the persistent,
+// grid-stride kernels, whose results do not depend on the grid size.
+inline int smCount() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return 1;
+  return n;
+}
 
 }  // namespace kb

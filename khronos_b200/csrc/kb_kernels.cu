@@ -1,4 +1,4 @@
-// Hand-written sm_100a kernels of the active-window fusion hot path.
+// Hand-written sm_90a kernels of the active-window fusion hot path.
 // Compile with -fmad=false: the per-voxel arithmetic must round exactly like the fp32 reference
 // (no FMA contraction), integer outputs (labels, indices, flags) are bit-exact by construction.
 //
@@ -589,7 +589,7 @@ __global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS
   int n_valid = 0, n_band = 0, n_sem = 0;
 
   // The cursor fetch for the NEXT item is issued before the current item is processed, so the atomic's
-  // L2 round trip (a quarter of all stall samples in profiles/r1_v5_*) overlaps useful work.
+  // L2 round trip overlaps useful work.
   int pending = 0;
   if (lane == 0) pending = atomicAdd(&m.counters[kFetch], 1);
   for (;;) {
@@ -1985,7 +1985,7 @@ __global__ void gatherSemanticKernel(const DeviceMap m, const int* slots, int L,
 }  // namespace
 
 void launchExpandFrames(const BatchParams& p, cudaStream_t s) {
-  expandFramesKernel<<<dim3(148, p.n_frames), 256, 0, s>>>(p);
+  expandFramesKernel<<<dim3(smCount(), p.n_frames), 256, 0, s>>>(p);
 }
 void launchExpandDepth(const uint16_t* src, float scale, float* dst, int n, cudaStream_t s) {
   expandDepthKernel<<<(n + 255) / 256, 256, 0, s>>>(src, scale, dst, n);
@@ -2103,7 +2103,7 @@ void launchHaloPack(const DeviceMap& m, const TrackingParams& p, const ShardExch
                     int32_t* halo_out, cudaStream_t s) {
   const int n = x.nranks * x.cap_pending * 27;
   haloMarkKernel<<<(n + 255) / 256, 256, 0, s>>>(m, x, all_pending);
-  haloPackKernel<<<148 * 4, kThreads, 0, s>>>(m, p, x, halo_out);
+  haloPackKernel<<<smCount() * 4, kThreads, 0, s>>>(m, p, x, halo_out);
   haloUnmarkKernel<<<(m.max_blocks + 255) / 256, 256, 0, s>>>(m, x, m.max_blocks);
 }
 void launchTrackingBeginPeers(const DeviceMap& m, const TrackingParams& p, const ShardExchange& x, const PeerBuffers& peers, cudaStream_t s) {
@@ -2114,13 +2114,13 @@ void launchHaloPackPeers(const DeviceMap& m, const TrackingParams& p, const Shar
                          const PeerBuffers& peers, cudaStream_t s) {
   const int n = x.nranks * x.cap_pending * 27;
   haloMarkKernel<<<(n + 255) / 256, 256, 0, s>>>(m, x, all_pending);
-  haloPackPeersKernel<<<148 * 4, kThreads, 0, s>>>(m, p, x, peers);
+  haloPackPeersKernel<<<smCount() * 4, kThreads, 0, s>>>(m, p, x, peers);
   haloUnmarkKernel<<<(m.max_blocks + 255) / 256, 256, 0, s>>>(m, x, m.max_blocks);
 }
 void launchMulticastCopy(void* mc_dst, const void* src, size_t bytes, cudaStream_t s) {
   const size_t n16 = bytes / 16;
   if (n16 == 0) return;
-  const int grid = static_cast<int>(std::min<size_t>((n16 + 255) / 256, 148 * 8));
+  const int grid = static_cast<int>(std::min<size_t>((n16 + 255) / 256, static_cast<size_t>(smCount()) * 8));
   multicastCopyKernel<<<grid, 256, 0, s>>>(static_cast<float4*>(mc_dst), static_cast<const float4*>(src), n16);
 }
 void launchFlagScatter(const uint8_t* local_flags, const PeerBuffers& peers, int n, cudaStream_t s) {

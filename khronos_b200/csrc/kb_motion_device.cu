@@ -282,12 +282,12 @@ void launchMotionClusteringSparse(const MotionTable& t, const int3* gidx, const 
   if (table_dirty) vtInitFullKernel<<<(cap + 255) / 256, 256, 0, s>>>(t);  // someone else used the table: full reset once
   else vtInitSparseKernel<<<1, 32, 0, s>>>(t);
   vtInsertKernel<<<(P + 255) / 256, 256, 0, s>>>(t, gidx, seed, P);
-  vtLinkKernel<<<148 * 4, 256, 0, s>>>(t, conn);
-  if (D > 1) vtMergeNearKernel<<<148 * 4, 256, 0, s>>>(t, D);
-  vtReduceSparseKernel<<<148, 256, 0, s>>>(t);
+  vtLinkKernel<<<smCount() * 4, 256, 0, s>>>(t, conn);
+  if (D > 1) vtMergeNearKernel<<<smCount() * 4, 256, 0, s>>>(t, D);
+  vtReduceSparseKernel<<<smCount(), 256, 0, s>>>(t);
   vtRankKernel<<<1, 1024, 0, s>>>(t, min_size, max_size);
   vtWriteImageKernel<<<(P + 255) / 256, 256, 0, s>>>(t, image, P);
-  vtCleanupKernel<<<148, 256, 0, s>>>(t);
+  vtCleanupKernel<<<smCount(), 256, 0, s>>>(t);
 }
 
 void launchMotionClustering(const MotionTable& t, const int3* gidx, const uint8_t* seed, int P, int conn, int D,
@@ -295,8 +295,8 @@ void launchMotionClustering(const MotionTable& t, const int3* gidx, const uint8_
   const int cap = static_cast<int>(t.mask) + 1;
   vtInitKernel<<<(cap + 255) / 256, 256, 0, s>>>(t);
   vtInsertKernel<<<(P + 255) / 256, 256, 0, s>>>(t, gidx, seed, P);
-  vtLinkKernel<<<148 * 4, 256, 0, s>>>(t, conn);     // persistent warps over the occupied-voxel list
-  if (D > 1) vtMergeNearKernel<<<148 * 4, 256, 0, s>>>(t, D);
+  vtLinkKernel<<<smCount() * 4, 256, 0, s>>>(t, conn);     // persistent warps over the occupied-voxel list
+  if (D > 1) vtMergeNearKernel<<<smCount() * 4, 256, 0, s>>>(t, D);
   vtReduceKernel<<<(cap + 255) / 256, 256, 0, s>>>(t);
   vtRankKernel<<<1, 1024, 0, s>>>(t, min_size, max_size);
   vtWriteImageKernel<<<(P + 255) / 256, 256, 0, s>>>(t, image, P);

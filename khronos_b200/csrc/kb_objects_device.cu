@@ -368,7 +368,7 @@ void launchObjectClustering3D(const MotionTable& t, const ObjectParams& p, cudaS
   const int cap = static_cast<int>(t.mask) + 1, P = p.W * p.H;
   osInitKernel<<<(cap + 255) / 256, 256, 0, s>>>(t);
   osInsertKernel<<<(P + 255) / 256, 256, 0, s>>>(t, p);
-  osLinkKernel<<<148 * 4, 256, 0, s>>>(t, p.full);
+  osLinkKernel<<<smCount() * 4, 256, 0, s>>>(t, p.full);
   osReduceKernel<<<(cap + 255) / 256, 256, 0, s>>>(t);
   osRankKernel<<<1, 1024, 0, s>>>(t, p.min_size, p.max_size);
   osWriteKernel<<<(P + 255) / 256, 256, 0, s>>>(t, p.image, P);

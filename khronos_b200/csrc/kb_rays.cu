@@ -628,7 +628,7 @@ int kb_rays_check(kb_ray_index* h, int32_t n_points, const float* points_xyz, co
   KR_CUDA(h, cudaMemcpyAsync(h->d_points, points_xyz, sizeof(float) * 3 * n_points, cudaMemcpyHostToDevice, h->stream));
   KR_CUDA(h, cudaMemcpyAsync(h->d_early, earliest, sizeof(uint64_t) * n_points, cudaMemcpyHostToDevice, h->stream));
   KR_CUDA(h, cudaMemcpyAsync(h->d_late, latest, sizeof(uint64_t) * n_points, cudaMemcpyHostToDevice, h->stream));
-  const int blocks = std::min((n_points + 7) / 8, 148 * 8);
+  const int blocks = std::min((n_points + 7) / 8, kb::smCount() * 8);
   const float inv_block = 1.f / h->cfg.block_size;
   rayCheckKernel<false><<<blocks, 256, 0, h->stream>>>(h->table, h->d_block_rays, h->d_src, h->d_dst, h->d_stamps, h->d_points, h->d_early, h->d_late, n_points, inv_block, h->cfg.radial_tolerance, h->cfg.depth_tolerance, h->d_pt_counts, nullptr, nullptr);
   KR_CUDA(h, cudaGetLastError());

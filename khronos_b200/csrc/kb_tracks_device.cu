@@ -140,7 +140,7 @@ void launchTrackIntersect(const MotionTable& t, const unsigned long long* track_
                           const int* present_ids, int n_present, int n_tracks, int* intersections, cudaStream_t s) {
   if (n_track_voxels <= 0 || n_present <= 0) return;
   const long long total = static_cast<long long>(n_track_voxels) * n_present;
-  const int blocks = static_cast<int>(total / 256 + 1 < 148 * 8 ? total / 256 + 1 : 148 * 8);
+  const int blocks = static_cast<int>(std::min<long long>(total / 256 + 1, smCount() * 8LL));
   tkIntersectKernel<<<blocks, 256, 0, s>>>(t, track_keys, track_of, n_track_voxels, present_ids, n_present, n_tracks, intersections);
 }
 
@@ -149,7 +149,7 @@ void launchVertexMap(const TrackParams& p, float* out, cudaStream_t s) {
 }
 
 void launchTrackExportKeys(const MotionTable& t, unsigned long long* out, cudaStream_t s) {
-  tkExportKernel<<<148, 256, 0, s>>>(t, out);
+  tkExportKernel<<<smCount(), 256, 0, s>>>(t, out);
 }
 
 }  // namespace kb

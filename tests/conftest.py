@@ -10,7 +10,7 @@ sys.path.insert(0, ROOT)
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # the synthetic renderer works on tiny tensors: intra-op threading only adds (large) overhead
     import torch
     torch.set_num_threads(1)

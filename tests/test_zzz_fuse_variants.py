@@ -1,5 +1,5 @@
 """Fuse-kernel variants, selected by environment variables read in kb_create. Since round 2 KB_PIPELINE, KB_FUSE_ITEM_LIST,
-KB_EVERFREE_V2 and KB_MOTION_SPARSE are ON by default (measured wins, profiles/r2_ab1_summary.txt), so the rest of the suite runs
+KB_EVERFREE_V2 and KB_MOTION_SPARSE are ON by default (they won the A/B runs), so the rest of the suite runs
 them and this file also runs the former defaults (=0); KB_FUSE_MLP and KB_H2D_NARROW_LABELS lost their A/Bs and stay off; KB_FUSE_COOP selects the CTA-cooperative two-phase fuse kernel:
   KB_FUSE_ITEM_LIST=1  items come from compacted heaviest-first lists instead of the dense box range
   KB_PIPELINE=1        the prologue (tile pyramid, K0, K0b) of batch i+1 runs on its own stream while the fuse kernel of

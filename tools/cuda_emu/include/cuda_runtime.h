@@ -4,7 +4,7 @@
 // only. Semantics: one OS thread; every CUDA thread of a block is a fiber (ucontext); fibers yield at warp / block
 // synchronising intrinsics and are resumed when all active lanes (threads) have arrived; blocks run one after the
 // other, so atomics are plain read-modify-writes and `__shared__` is a function-local static. Nothing about timing,
-// memory spaces, races or sm_100a code generation is modelled. The product never loads this library.
+// memory spaces, races or sm_90a code generation is modelled. The product never loads this library.
 #pragma once
 #define __CUDACC__ 1
 #define KB_CUDA_EMU 1

@@ -10,8 +10,8 @@ checked against the oracle in a container without a GPU:
 
 What this proves: the arithmetic, indexing, hashing, work distribution and synchronisation structure of the kernels
 give the oracle's results when executed with CUDA's thread / warp / block semantics (one fiber per CUDA thread).
-What it cannot prove: anything about real concurrency (races between warps or blocks), memory spaces, sm_100a code
-generation or speed — the -m gpu run on a B200 remains the parity gate. The emulated library is never shipped and
+What it cannot prove: anything about real concurrency (races between warps or blocks), memory spaces, sm_90a code
+generation or speed — the -m gpu run on an H100 remains the parity check. The emulated library is never shipped and
 the product package never loads it (khronos_b200.lib() is monkeypatched in this process only)."""
 import ctypes
 import os
