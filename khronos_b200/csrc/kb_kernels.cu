@@ -534,7 +534,10 @@ __device__ __forceinline__ int listedBox(const BatchParams& p, const int (&n_cls
 // ---- K1: projective TSDF + semantic fusion ----------------------------------------------------------------
 // Lazy tracking fold (see evalTracking): what the tracking passes since the voxel's last write would have
 // done to it. Returns the flag byte to carry (ever_free, active, to_remove); refreshes last_occupied.
-__device__ __noinline__ uint32_t trackingFold(const DeviceMap m, const TrackEval t, uint32_t born, size_t gi) {
+// Out of line so that the fuse kernel's item loop keeps its register budget. The arguments are references into the
+// calling kernel's __grid_constant__ parameters: passed by value, the DeviceMap (~200 B) and TrackEval would be copied to
+// the stack at every call, i.e. once per voxel and batch.
+__device__ __noinline__ uint32_t trackingFold(const DeviceMap& m, const TrackEval& t, uint32_t born, size_t gi) {
   const uint8_t fl = m.vflags[gi];
   const uint32_t c_stored = m.last_occ[gi];
   uint32_t c_true;
@@ -560,7 +563,7 @@ __device__ __noinline__ uint32_t trackingFold(const DeviceMap m, const TrackEval
 // LIST: items come from the compacted, heaviest-first box lists of itemCompactKernel instead of the dense box range.
 // PB: the batch uses the second cursor / item-list counter set (odd batches of KB_PIPELINE).
 template <int VPS, int LPI, bool COMPACT, bool COLOR, bool LIST = false, bool PB = false>
-__global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS : KB_FUSE_MIN_BLOCKS) fuseKernel(const DeviceMap m, const __grid_constant__ BatchParams p) {
+__global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS : KB_FUSE_MIN_BLOCKS) fuseKernel(const __grid_constant__ DeviceMap m, const __grid_constant__ BatchParams p) {
   constexpr int kFetch = PB ? kCtrFetchB : kCtrFetch;
   [[maybe_unused]] constexpr int kItems = PB ? kCtrItemsB0 : kCtrItems0;
   constexpr int V = VPS * VPS * VPS;
@@ -807,7 +810,7 @@ __global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS
 // voxel, so results are bit-identical; the chain per item shrinks to a quarter of the frames plus a short fold, and the
 // scheduling unit becomes the CTA (~15 items each instead of ~4 per warp).
 template <int VPS, bool COMPACT, bool PB>
-__global__ void __launch_bounds__(kFuseThreads, KB_FUSE_MIN_BLOCKS) fuseKernelCoop(const DeviceMap m, const __grid_constant__ BatchParams p) {
+__global__ void __launch_bounds__(kFuseThreads, KB_FUSE_MIN_BLOCKS) fuseKernelCoop(const __grid_constant__ DeviceMap m, const __grid_constant__ BatchParams p) {
   constexpr int kFetch = PB ? kCtrFetchB : kCtrFetch;
   constexpr int kItems = PB ? kCtrItemsB0 : kCtrItems0;
   constexpr int V = VPS * VPS * VPS;
@@ -1044,7 +1047,7 @@ __global__ void __launch_bounds__(kFuseThreads, KB_FUSE_MIN_BLOCKS) fuseKernelCo
 #define KB_FUSE_MLP_MIN_BLOCKS 5
 #endif
 template <int VPS, int LPI, bool COMPACT, int G, bool LIST, bool PB = false>
-__global__ void __launch_bounds__(kFuseThreads, KB_FUSE_MLP_MIN_BLOCKS) fuseKernelMlp(const DeviceMap m, const __grid_constant__ BatchParams p) {
+__global__ void __launch_bounds__(kFuseThreads, KB_FUSE_MLP_MIN_BLOCKS) fuseKernelMlp(const __grid_constant__ DeviceMap m, const __grid_constant__ BatchParams p) {
   constexpr int kFetch = PB ? kCtrFetchB : kCtrFetch;
   [[maybe_unused]] constexpr int kItems = PB ? kCtrItemsB0 : kCtrItems0;
   constexpr int V = VPS * VPS * VPS;
