@@ -16,6 +16,8 @@ import pytest
 from khronos_b200 import capi, synthetic as syn
 import harness as hs
 from test_parity_gpu import room_frames
+import test_zzz_long_calls as tlc
+from test_zzz_long_calls import hall_oracle  # noqa: F401  (fixture: the oracle's map of the long stream, once per session)
 
 pytestmark = pytest.mark.gpu
 
@@ -28,6 +30,16 @@ VARIANTS = [{"KB_FUSE_MLP": "2"}, {"KB_FUSE_MLP": "4", "KB_FUSE_ITEM_LIST": "1",
 
 @pytest.fixture(params=VARIANTS, ids=lambda v: "+".join(f"{k.replace('KB_', '').replace('FUSE_', '')}={x}" for k, x in v.items()))
 def variant_env(request):
+    os.environ.update(request.param)   # read by kb_create
+    yield request.param
+    for k in request.param:
+        os.environ.pop(k, None)
+
+
+@pytest.fixture(params=[{}] + VARIANTS + [{"KB_FUSE_CTAS_PER_SM": "1"}],
+                ids=lambda v: "+".join(f"{k.replace('KB_', '').replace('FUSE_', '')}={x}" for k, x in v.items()) or "default")
+def long_variant_env(request):
+    """The defaults, every variant, and one fuse CTA per SM (longer fuse kernels widen the window the prologue overlaps)."""
     os.environ.update(request.param)   # read by kb_create
     yield request.param
     for k in request.param:
@@ -201,3 +213,12 @@ def test_everfree_v2_variant(oracle_lib, product_lib, v2):
             hs.assert_blocks_equal(bo, g.export_blocks(), exact_float=True, what=f"everfree v2 conn {conn}")
     finally:
         os.environ.pop("KB_EVERFREE_V2", None)
+
+
+@pytest.mark.gpu(slow=True)
+def test_variant_long_pipelined_call_equals_oracle(product_lib, hall_oracle, long_variant_env):
+    """The benchmark's call shape (test_zzz_long_calls: ~1000 hall640 frames in one call on a caller stream, then the
+    revisit) under every fuse variant, against the oracle's map computed once for all of them."""
+    g, sched = tlc.run_long_calls(product_lib, 19)
+    sched.assert_covers()
+    tlc.assert_matches_oracle(g, hall_oracle, f"long call {long_variant_env}")
