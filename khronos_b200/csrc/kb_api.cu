@@ -110,6 +110,7 @@ struct kb_handle {
   std::vector<int32_t> h_pixel_gidx;
   std::vector<uint8_t> h_pixel_seed;
   std::vector<float> h_depth;
+  std::vector<float> h_vertex;  // host copy of a device-resident caller vertex map (cluster bounding boxes)
   MotionResult motion;
   MotionTable mt{};            // device clustering table (M2-M4)
   int32_t* d_dynamic = nullptr;  // device copy of the last dynamic image (usable as KB_MASK_LAST_DETECTION)
@@ -321,7 +322,8 @@ int ensureMotionBuffers(kb_handle* h, size_t pixels) {
   uint32_t cap = 1024;
   while (cap < 2 * pixels) cap <<= 1;
   t.mask = cap - 1;
-  t.max_roots = 4096;
+  // every root is an occupied slot and at most one slot per pixel is occupied, so the root list never overflows
+  t.max_roots = static_cast<int>(pixels);
   KB_CUDA(h, devAlloc(&t.keys, cap, 0xFF));
   KB_CUDA(h, devAlloc(&t.count, cap, 0));
   KB_CUDA(h, devAlloc(&t.flags, cap, 0));
@@ -409,8 +411,9 @@ int slotHwm(kb_handle* h, int* n) {
 }
 
 // Host M2-M4 on the per-pixel voxel keys of the last M1 launch (slow path: cluster lists on demand, separation
-// distance <= 0, caller-supplied vertex maps, pathological cluster counts).
-int buildMotionClustersOnHost(kb_handle* h, const float* vertex_world_host, int32_t* image_out) {
+// distance <= 0, caller-supplied vertex maps). A caller vertex map in device memory is copied back with the other M1
+// inputs: the bounding boxes come from the vertex map, not from the back-projected depth (:396-397).
+int buildMotionClustersOnHost(kb_handle* h, const float* vertex_world, bool vertex_on_device, int32_t* image_out) {
   const size_t px = static_cast<size_t>(h->cam.width) * h->cam.height;
   h->h_pixel_gidx.resize(px * 3);
   h->h_pixel_seed.resize(px);
@@ -418,10 +421,15 @@ int buildMotionClustersOnHost(kb_handle* h, const float* vertex_world_host, int3
   KB_CUDA(h, cudaMemcpyAsync(h->h_pixel_gidx.data(), h->d_pixel_gidx, sizeof(int3) * px, cudaMemcpyDeviceToHost, h->stream));
   KB_CUDA(h, cudaMemcpyAsync(h->h_pixel_seed.data(), h->d_pixel_seed, px, cudaMemcpyDeviceToHost, h->stream));
   KB_CUDA(h, cudaMemcpyAsync(h->h_depth.data(), h->mot_depth, sizeof(float) * px, cudaMemcpyDeviceToHost, h->stream));
+  if (vertex_world && vertex_on_device) {
+    h->h_vertex.resize(px * 3);
+    KB_CUDA(h, cudaMemcpyAsync(h->h_vertex.data(), vertex_world, sizeof(float) * 3 * px, cudaMemcpyDeviceToHost, h->stream));
+    vertex_world = h->h_vertex.data();
+  }
   KB_CUDA(h, cudaStreamSynchronize(h->stream));
   std::vector<int32_t> scratch;
   if (!image_out) { scratch.assign(px, 0); image_out = scratch.data(); }
-  clusterMotion(h->motion_hp, h->h_pixel_gidx.data(), h->h_pixel_seed.data(), h->h_depth.data(), vertex_world_host,
+  clusterMotion(h->motion_hp, h->h_pixel_gidx.data(), h->h_pixel_seed.data(), h->h_depth.data(), vertex_world,
                 image_out, &h->motion);
   h->motion_stale = false;
   return KB_OK;
@@ -1686,18 +1694,13 @@ int kb_detect_motion(kb_handle* h, const kb_frame* f, int32_t* dynamic_image_out
       if ((st = enqueueDeviceClustering(h)) != KB_OK) return st;
       KB_CUDA(h, cudaMemcpyAsync(dynamic_image_out, h->d_dynamic, sizeof(int32_t) * px, cudaMemcpyDeviceToHost, h->stream));
       KB_CUDA(h, cudaStreamSynchronize(h->stream));
-      if (h->h_mscal[kMsRoots] > h->mt.max_roots) {
-        device_path = false;  // pathological number of clusters: fall through to the host path
-      } else {
-        h->motion.n_seeds = h->h_mscal[kMsSeeds];
-        n_clusters_out = h->h_mscal[kMsClusters];
-        h->motion_stale = n_clusters_out > 0;  // cluster lists are built on demand (kb_get_motion_clusters)
-        h->motion_have_image = true;
-      }
-    }
-    if (!device_path) {
+      h->motion.n_seeds = h->h_mscal[kMsSeeds];
+      n_clusters_out = h->h_mscal[kMsClusters];
+      h->motion_stale = n_clusters_out > 0;  // cluster lists are built on demand (kb_get_motion_clusters)
+      h->motion_have_image = true;
+    } else {
       std::memset(dynamic_image_out, 0, sizeof(int32_t) * px);
-      if ((st = buildMotionClustersOnHost(h, f->memory == KB_MEM_DEVICE ? nullptr : f->vertex_world, dynamic_image_out)) != KB_OK) return st;
+      if ((st = buildMotionClustersOnHost(h, f->vertex_world, f->memory == KB_MEM_DEVICE, dynamic_image_out)) != KB_OK) return st;
       n_clusters_out = static_cast<int>(h->motion.clusters.size());
       KB_CUDA(h, cudaMemcpyAsync(h->d_dynamic, dynamic_image_out, sizeof(int32_t) * px, cudaMemcpyHostToDevice, h->stream));
       h->motion_have_image = true;
@@ -1738,7 +1741,6 @@ int kb_spin_once(kb_handle* h, const kb_frame* f, int32_t* dynamic_image_out, in
   if ((st = kb_integrate_frames(h, &g, 1, 1, nullptr)) != KB_OK) return st;
   if ((st = updateTrackingImpl(h, f->stamp_ns)) != KB_OK) return st;
   KB_CUDA(h, cudaStreamSynchronize(h->stream));
-  if (h->h_mscal[kMsRoots] > h->mt.max_roots) return fail(h, KB_ERR_CAPACITY, "too many motion clusters for the device path");
   h->motion.n_seeds = h->h_mscal[kMsSeeds];
   h->motion_stale = h->h_mscal[kMsClusters] > 0;
   if (n_seeds) *n_seeds = h->h_mscal[kMsSeeds];
@@ -1756,7 +1758,10 @@ int kb_detect_objects(kb_handle* h, const kb_object_detector_config* cfg, const 
   const size_t px = static_cast<size_t>(c.width) * c.height;
   int st;
   if ((st = ensureObjectBuffers(h, px)) != KB_OK) return st;
-  if (h->mt.max_roots * 1024 < static_cast<int>(px)) return fail(h, KB_ERR_CAPACITY, "image too large for the 2D scan");
+  // the object ranking stays bounded (single-CTA O(n^2) rank): more semantic clusters than this is a capacity error
+  MotionTable ot = h->mt;
+  ot.max_roots = std::min(ot.max_roots, 4096);
+  if (ot.max_roots * 1024 < static_cast<int>(px)) return fail(h, KB_ERR_CAPACITY, "image too large for the 2D scan");
   h->obj_have = false;
   if (!f->label && !f->label_u8) {  // no semantic image: no objects (connected_semantics.cpp reads label_image only)
     std::memset(object_image_out, 0, sizeof(int32_t) * px);
@@ -1802,15 +1807,15 @@ int kb_detect_objects(kb_handle* h, const kb_object_detector_config* cfg, const 
     else std::memcpy(h->obj_label_host.data(), f->label, sizeof(int) * px);
   }
   if (cfg->use_3d && (st = stage(h, f->vertex_world, h->stg_vertex, px * 3, f->memory, &p.vertex)) != KB_OK) return st;
-  if (cfg->use_3d) launchObjectClustering3D(h->mt, p, h->stream);
-  else launchObjectClustering2D(h->mt, p, h->stream);
+  if (cfg->use_3d) launchObjectClustering3D(ot, p, h->stream);
+  else launchObjectClustering2D(ot, p, h->stream);
   h->mt_dirty = true;  // shared table memory
   h->trk_have = false;
   KB_CUDA(h, cudaGetLastError());
   KB_CUDA(h, cudaMemcpyAsync(h->h_oscal, h->mt.scalars, sizeof(int) * kMsCount, cudaMemcpyDeviceToHost, h->stream));
   KB_CUDA(h, cudaMemcpyAsync(object_image_out, h->d_object, sizeof(int32_t) * px, cudaMemcpyDeviceToHost, h->stream));
   KB_CUDA(h, cudaStreamSynchronize(h->stream));
-  if (cfg->use_3d && h->h_oscal[kMsRoots] > h->mt.max_roots)
+  if (cfg->use_3d && h->h_oscal[kMsRoots] > ot.max_roots)
     return fail(h, KB_ERR_CAPACITY, "too many semantic clusters for the device ranking");
   h->obj_image_host.assign(object_image_out, object_image_out + px);
   h->obj_have = true;
@@ -2213,7 +2218,6 @@ int kb_motion_result(kb_handle* h, int32_t* dynamic_image_out, int32_t* n_seeds,
   if (dynamic_image_out)
     KB_CUDA(h, cudaMemcpyAsync(dynamic_image_out, h->d_dynamic, sizeof(int32_t) * px, cudaMemcpyDeviceToHost, h->stream));
   KB_CUDA(h, cudaStreamSynchronize(h->stream));
-  if (h->h_mscal[kMsRoots] > h->mt.max_roots) return fail(h, KB_ERR_CAPACITY, "too many motion clusters for the device path");
   h->motion.n_seeds = h->h_mscal[kMsSeeds];
   h->motion_stale = h->h_mscal[kMsClusters] > 0;
   if (n_seeds) *n_seeds = h->h_mscal[kMsSeeds];
@@ -2254,7 +2258,7 @@ int kb_get_motion_clusters(kb_handle* h, int32_t* counts, int32_t* pixels_uv, in
   if (!h) return KB_ERR_INVALID;
   if (h->motion_stale) {
     KB_CUDA(h, cudaSetDevice(h->device));
-    const int st = buildMotionClustersOnHost(h, nullptr, nullptr);
+    const int st = buildMotionClustersOnHost(h, nullptr, false, nullptr);
     if (st != KB_OK) return st;
   }
   size_t tp = 0, tv = 0;

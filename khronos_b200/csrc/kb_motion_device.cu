@@ -166,7 +166,9 @@ __global__ void vtReduceKernel(MotionTable t) {
   }
 }
 
-// C5: size filter + ranking by smallest seed -> cluster ids (single CTA; clusters are few).
+// C5: size filter + ranking by smallest seed -> cluster ids. Single CTA, quadratic in the number of roots: cheap for the
+// usual handful of clusters; a frame with thousands of isolated components (up to one root per pixel) pays n^2 / 1024
+// steps per thread, which only pathological frames reach.
 __global__ void vtRankKernel(MotionTable t, int min_size, int max_size) {
   if (*t.gate == 0) return;
   const int n = min(t.scalars[kMsRoots], t.max_roots);
