@@ -2,7 +2,7 @@
 The reference's mesher lives in un-vendored Hydra (parity unpinned); what can be pinned is pinned here:
   * both copies of the 256-case table (product + oracle) are identical, every row uses exactly the cube edges whose end
     points differ in sign, and meshes of random sign fields are closed, 2-manifold and consistently oriented;
-  * the oracle's mesh equals an independent numpy restatement of the spec on its own exported TSDF (bit-exact vertices);
+  * the oracle's mesh equals the from-spec model (mesh_model.py) on its own exported TSDF (bit-exact vertices, colours, labels);
   * geometry: the mesh of a fused flat wall lies on the wall, faces the camera side, and its area matches."""
 import os
 import re
@@ -13,6 +13,7 @@ import pytest
 
 from khronos_b200 import capi, synthetic as syn
 import harness as hs
+import mesh_model as mm
 
 EDGES = [(0, 1), (1, 2), (2, 3), (3, 0), (4, 5), (5, 6), (6, 7), (7, 4), (0, 4), (1, 5), (2, 6), (3, 7)]
 OFFS = [(0, 0, 0), (1, 0, 0), (1, 1, 0), (0, 1, 0), (0, 0, 1), (1, 0, 1), (1, 1, 1), (0, 1, 1)]
@@ -69,80 +70,6 @@ def test_table_meshes_are_closed_manifold_and_oriented():
             assert cnt == 1 and directed.get((b, a), 0) == 1
 
 
-def numpy_mesh(blocks: capi.Blocks, voxel_size, vps, min_weight=1e-4, only=None):
-    """Spec restatement (docs/ORACLE_SPEC.md §13) on an exported map: list of (block index, points (n,3) f32, labels)."""
-    f32 = np.float32
-    V = vps ** 3
-    idx = {tuple(b): i for i, b in enumerate(blocks.block_index.reshape(-1, 3).tolist())}
-    bs = f32(voxel_size) * f32(vps)
-    m = vps - 1
-    order = ([(x, y, z) for x in range(m) for y in range(m) for z in range(m)] + [(m, y, z) for z in range(vps) for y in range(vps)] +
-             [(x, m, z) for z in range(vps) for x in range(m)] + [(x, y, m) for y in range(m) for x in range(m)])
-    out = []
-    for b in sorted(idx):
-        if only is not None and b not in only:
-            continue
-        D = np.zeros((vps + 1,) * 3, f32)
-        Wt = np.full((vps + 1,) * 3, -1.0, f32)
-        LB = np.zeros((vps + 1,) * 3, np.uint32)
-        for dz in (0, 1):
-            for dy in (0, 1):
-                for dx in (0, 1):
-                    nb = (b[0] + dx, b[1] + dy, b[2] + dz)
-                    if nb not in idx:
-                        continue
-                    i = idx[nb]
-                    d = blocks.distance[i].reshape(vps, vps, vps).transpose(2, 1, 0)  # [x, y, z]
-                    w = blocks.weight[i].reshape(vps, vps, vps).transpose(2, 1, 0)
-                    lb = np.where(blocks.semantic_empty[i] != 0, 0, blocks.semantic_label[i]).reshape(vps, vps, vps).transpose(2, 1, 0)
-                    sx = slice(0, vps) if dx == 0 else slice(vps, vps + 1)
-                    sy = slice(0, vps) if dy == 0 else slice(vps, vps + 1)
-                    sz = slice(0, vps) if dz == 0 else slice(vps, vps + 1)
-                    D[sx, sy, sz] = d[(slice(0, vps) if dx == 0 else slice(0, 1)), (slice(0, vps) if dy == 0 else slice(0, 1)), (slice(0, vps) if dz == 0 else slice(0, 1))]
-                    Wt[sx, sy, sz] = w[(slice(0, vps) if dx == 0 else slice(0, 1)), (slice(0, vps) if dy == 0 else slice(0, 1)), (slice(0, vps) if dz == 0 else slice(0, 1))]
-                    LB[sx, sy, sz] = lb[(slice(0, vps) if dx == 0 else slice(0, 1)), (slice(0, vps) if dy == 0 else slice(0, 1)), (slice(0, vps) if dz == 0 else slice(0, 1))]
-        ok = np.ones((vps,) * 3, bool)
-        case = np.zeros((vps,) * 3, np.int32)
-        for c, (ox, oy, oz) in enumerate(OFFS):
-            sl = (slice(ox, ox + vps), slice(oy, oy + vps), slice(oz, oz + vps))
-            ok &= Wt[sl] >= f32(min_weight)
-            case |= (D[sl] < 0).astype(np.int32) << c
-        case[~ok] = 0
-        case[case == 255] = 0
-        pts, labs = [], []
-        if case.any():
-            for (x, y, z) in order:
-                c = int(case[x, y, z])
-                if not c:
-                    continue
-                pos, sdf, lab = [], [], []
-                for (ox, oy, oz) in OFFS:
-                    vx, vy, vz = x + ox, y + oy, z + oz
-                    bx, by, bz = b[0] + (vx == vps), b[1] + (vy == vps), b[2] + (vz == vps)
-                    lx, ly, lz = vx % vps, vy % vps, vz % vps
-                    pos.append(np.array([f32(bx) * bs + (f32(lx) + f32(0.5)) * f32(voxel_size), f32(by) * bs + (f32(ly) + f32(0.5)) * f32(voxel_size),
-                                         f32(bz) * bs + (f32(lz) + f32(0.5)) * f32(voxel_size)], f32))
-                    sdf.append(D[vx, vy, vz])
-                    lab.append(LB[vx, vy, vz])
-                row = TABLE[c]
-                k = 0
-                while k < 16 and row[k] >= 0:
-                    for e in (row[k + 2], row[k + 1], row[k]):
-                        c0, c1 = EDGES[e]
-                        diff = f32(sdf[c0] - sdf[c1])
-                        if abs(diff) >= f32(1e-6):
-                            t = f32(sdf[c0] / diff)
-                            v = (pos[c0] + t * (pos[c1] - pos[c0])).astype(f32)
-                        else:
-                            t = f32(0.5)
-                            v = (f32(0.5) * (pos[c0] + pos[c1])).astype(f32)
-                        pts.append(v)
-                        labs.append(lab[c0] if t < f32(0.5) else lab[c1])
-                    k += 3
-        out.append((b, np.array(pts, f32).reshape(-1, 3), np.array(labs, np.uint32)))
-    return out
-
-
 def _room(n=5, scale=8):
     cam = hs.small_camera(scale)
     scene = syn.room_scene()
@@ -155,12 +82,13 @@ def test_oracle_mesh_equals_numpy_restatement(oracle_lib):
     o = hs.make_handle(oracle_lib, "ko_", cam=cam)
     hs.run_fusion(o, frames, poses, stamps)
     bi, off, pts, col, lab = o.generate_mesh(only_mesh_updated=False, clear_updated_flag=False)
-    ref = numpy_mesh(o.export_blocks(), 0.05, 16)
-    assert len(ref) == len(bi) and off[-1] == len(pts) and len(pts) % 3 == 0 and len(pts) > 3000
-    for i, (b, p, l) in enumerate(ref):
-        assert tuple(bi[i]) == b
-        np.testing.assert_array_equal(pts[off[i]:off[i + 1]].view(np.uint32), p.view(np.uint32), err_msg=f"block {b}")
-        np.testing.assert_array_equal(lab[off[i]:off[i + 1]], l)
+    ref = mm.mesh(o.export_blocks(), 0.05, 16, TABLE)
+    assert len(ref.block_index) == len(bi) and off[-1] == len(pts) and len(pts) % 3 == 0 and len(pts) > 3000
+    np.testing.assert_array_equal(bi, ref.block_index)
+    np.testing.assert_array_equal(off, ref.offsets)
+    np.testing.assert_array_equal(pts.view(np.uint32), ref.points.view(np.uint32))
+    np.testing.assert_array_equal(col, ref.colors)
+    np.testing.assert_array_equal(lab, ref.labels)
 
 
 def test_mesh_updated_flag_semantics(oracle_lib):
