@@ -1189,6 +1189,19 @@ static int integrateBatch(kb_handle* h, const kb_frame* frames, int n, int alloc
   bool all_compact = any_compact;
   for (int b = 0; b < n; ++b) all_compact = all_compact && frames[b].depth_u16 != nullptr && frames[b].label == nullptr;
   p.compact_taps = all_compact ? 1 : 0;
+  // Per-frame image presence as bit words, so the fuse kernel's frame loop tests one bit instead of loading pointers. The
+  // label image a frame is read through: the object image in BINARY mode, else the u8 labels of an all-compact batch
+  // (read in place) or the i32 ones (caller's, staged, or expanded from u8).
+  p.label_frames = 0;
+  p.mask_frames = 0;
+  for (int b = 0; b < n; ++b) {
+    const FrameView& v = p.f[b];
+    const void* lab = p.sem_mode == KB_SEMANTICS_BINARY ? static_cast<const void*>(v.object_image)
+                      : all_compact                     ? static_cast<const void*>(v.label8)
+                                                        : static_cast<const void*>(v.label);
+    if (p.L > 0 && lab != nullptr) p.label_frames |= 1u << b;
+    if (v.mask != nullptr) p.mask_frames |= 1u << b;
+  }
   cudaStream_t ps = h->stream;
   if (pipe) {
     // The prologue of this batch goes to its own stream: it may run while the previous batch's fuse kernel is still

@@ -25,6 +25,10 @@ namespace {
 
 constexpr int kThreads = 256;
 constexpr int kFuseThreads = 128;  // 4 independent warps per CTA
+// Floats per thread of fuseKernel's likelihood rows (s_rows[thread][S]): Lp rounded up to an odd multiple of 4, so the
+// 16 B row accesses of a quarter-warp (8 lanes) fall on 8 disjoint groups of 4 banks. BINARY rows (Lp = 2) keep the
+// transposed [2][thread] layout.
+__host__ __device__ constexpr int fuseRowStride(int Lp) { return Lp <= 2 ? 2 : ((Lp >> 2) | 1) << 2; }
 #ifndef KB_FUSE_MIN_BLOCKS
 #define KB_FUSE_MIN_BLOCKS 10      // resident CTAs per SM the fuse kernel is compiled for (register cap 65536/(128*N))
 #endif
@@ -550,7 +554,7 @@ __device__ __noinline__ uint32_t trackingFold(const DeviceMap& m, const TrackEva
 // Persistent warps fetch work items from a shared cursor. An item = one z-layer (4x8 voxels, one per lane) of
 // a 4x8x4 box that survived culling, together with the box's frame mask. The lane keeps its voxel's
 // {distance, weight, last_observed, flags} in registers and its semantic likelihood row in shared memory
-// (transposed [label][thread]: conflict free) while the warp walks the surviving frames in order: TSDF and
+// ([thread][fuseRowStride(Lp)]: moved with conflict-free 16 B accesses) while the warp walks the surviving frames in order: TSDF and
 // likelihoods are read and written once per batch, every warp access covers whole 32 B sectors, and the
 // serial dependency chain per item is one voxel deep, so ~25 k items per batch balance over the SMs.
 // Warps never synchronise with each other.
@@ -569,7 +573,8 @@ __global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS
   constexpr int V = VPS * VPS * VPS;
   constexpr int NK = 4;                                      // z-layers per culling box
   constexpr int BOXES = (VPS / 4) * (VPS / 8) * (VPS / NK);  // 32 (16^3) or 4 (8^3) boxes of 128 voxels
-  extern __shared__ float s_rows[];                          // [Lp][kFuseThreads] likelihood rows
+  extern __shared__ float4 s_rows4[];                        // [kFuseThreads][S] likelihood rows (BINARY: [2][kFuseThreads])
+  float* const s_rows = reinterpret_cast<float*>(s_rows4);
   const int lane = threadIdx.x & 31;
   // Short batches have little work per voxel, so an item then covers all NK layers of its box (amortising the
   // fetch); long batches use one layer per item for balance.
@@ -633,7 +638,7 @@ __global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS
       const int b = __ffs(rem) - 1;
       rem &= rem - 1;
       const FrameView& f = p.f[b];
-      const bool has_label_img = L > 0 && (binary ? f.object_image != nullptr : (COMPACT ? f.label8 != nullptr : f.label != nullptr));
+      const bool has_label_img = (p.label_frames >> b) & 1u;
       float x, y, z;
       xform(f.R, f.t, wx, wy, wz, x, y, z);
       if (z <= 0.f) continue;
@@ -649,7 +654,7 @@ __global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS
       uint32_t label = 0;
       if (in_band) {
         const int ti = tapIndex(p, taps);  // interpolateID: the pixel of the dominant tap
-        if (f.mask != nullptr && __ldg(&f.mask[ti]) != 0) continue;
+        if (((p.mask_frames >> b) & 1u) && __ldg(&f.mask[ti]) != 0) continue;
         if (has_label_img) {
           if (binary) {
             label = __ldg(&f.object_image[ti]) == f.target_id ? 1u : 0u;
@@ -697,12 +702,12 @@ __global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS
             s_rows[kFuseThreads + threadIdx.x] = c.y;
           } else {
             const float4* __restrict__ lk = reinterpret_cast<const float4*>(m.sem_lik + si * m.Lp);
-            for (int k4 = 0; k4 < m.Lp; k4 += 4) {
-              const float4 c = empty ? make_float4(p.mle_init, p.mle_init, p.mle_init, p.mle_init) : lk[k4 >> 2];
-              s_rows[(k4 + 0) * kFuseThreads + threadIdx.x] = c.x;
-              s_rows[(k4 + 1) * kFuseThreads + threadIdx.x] = c.y;
-              s_rows[(k4 + 2) * kFuseThreads + threadIdx.x] = c.z;
-              s_rows[(k4 + 3) * kFuseThreads + threadIdx.x] = c.w;
+            float4* const row = s_rows4 + threadIdx.x * (fuseRowStride(m.Lp) >> 2);
+            const float4 init = make_float4(p.mle_init, p.mle_init, p.mle_init, p.mle_init);
+#pragma unroll
+            for (int q = 0; q < KB_MAX_LABELS / 4; ++q) {
+              if (4 * q >= m.Lp) break;
+              row[q] = empty ? init : lk[q];
             }
           }
         }
@@ -711,16 +716,26 @@ __global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS
           s_rows[label * kFuseThreads + threadIdx.x] = c;
           best_label = s_rows[kFuseThreads + threadIdx.x] > s_rows[threadIdx.x] ? 1 : 0;
         } else {
-          // likelihoods += logM[:, label]: two independent shared-memory read-modify-writes per step (entries beyond L are
-          // padding that nobody reads); the arg max is taken once, when the row is written back — only its final value
-          // is ever stored, and it only depends on the final row
-          for (int k2 = 0; k2 < m.Lp; k2 += 2) {
-            float c0 = s_rows[(k2 + 0) * kFuseThreads + threadIdx.x], c1 = s_rows[(k2 + 1) * kFuseThreads + threadIdx.x];
-            c0 += static_cast<uint32_t>(k2 + 0) == label ? p.mle_diag : p.mle_off;
-            c1 += static_cast<uint32_t>(k2 + 1) == label ? p.mle_diag : p.mle_off;
-            s_rows[(k2 + 0) * kFuseThreads + threadIdx.x] = c0;
-            s_rows[(k2 + 1) * kFuseThreads + threadIdx.x] = c1;
+          // likelihoods += logM[:, label], i.e. mle_off on every entry but the label's, which gets mle_diag. Every entry
+          // still receives exactly one addition per frame: the label entry is read first, the whole row (padding included,
+          // which nobody reads) takes mle_off in 16 B steps, then the label entry is overwritten with old + mle_diag.
+          // The arg max is taken once, when the row is written back — only its final value is ever stored, and it only
+          // depends on the final row.
+          float* const row = s_rows + threadIdx.x * fuseRowStride(m.Lp);
+          float4* const row4 = reinterpret_cast<float4*>(row);
+          const float c_label = row[label];
+          const float off = p.mle_off;
+#pragma unroll
+          for (int q = 0; q < KB_MAX_LABELS / 4; ++q) {
+            if (4 * q >= m.Lp) break;
+            float4 c = row4[q];
+            c.x += off;
+            c.y += off;
+            c.z += off;
+            c.w += off;
+            row4[q] = c;
           }
+          row[label] = c_label + p.mle_diag;
         }
         ++n_sem;
       }
@@ -741,17 +756,22 @@ __global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS
         if (binary) {
           *reinterpret_cast<float2*>(m.sem_lik + si * 2) = make_float2(s_rows[threadIdx.x], s_rows[kFuseThreads + threadIdx.x]);
         } else {
+          // SemanticVoxel::semantic_label = first maximum of the final likelihoods over 0..L-1 (UP App. A.8), taken from
+          // the values being written back
           float4* __restrict__ lk = reinterpret_cast<float4*>(m.sem_lik + si * m.Lp);
-          for (int k4 = 0; k4 < m.Lp; k4 += 4)
-            lk[k4 >> 2] = make_float4(s_rows[(k4 + 0) * kFuseThreads + threadIdx.x], s_rows[(k4 + 1) * kFuseThreads + threadIdx.x],
-                                      s_rows[(k4 + 2) * kFuseThreads + threadIdx.x], s_rows[(k4 + 3) * kFuseThreads + threadIdx.x]);
-        }
-        if (!binary) {  // SemanticVoxel::semantic_label = first maximum of the final likelihoods (UP App. A.8)
-          float bestv = s_rows[threadIdx.x];
+          const float4* const row = s_rows4 + threadIdx.x * (fuseRowStride(m.Lp) >> 2);
+          float bestv = 0.f;
           best_label = 0;
-          for (int kk = 1; kk < L; ++kk) {
-            const float c = s_rows[kk * kFuseThreads + threadIdx.x];
-            if (c > bestv) { bestv = c; best_label = kk; }
+#pragma unroll
+          for (int q = 0; q < KB_MAX_LABELS / 4; ++q) {
+            if (4 * q >= m.Lp) break;
+            const float4 c = row[q];
+            lk[q] = c;
+            if (q == 0) bestv = c.x;
+            else if (4 * q < L && c.x > bestv) { bestv = c.x; best_label = 4 * q; }
+            if (4 * q + 1 < L && c.y > bestv) { bestv = c.y; best_label = 4 * q + 1; }
+            if (4 * q + 2 < L && c.z > bestv) { bestv = c.z; best_label = 4 * q + 2; }
+            if (4 * q + 3 < L && c.w > bestv) { bestv = c.w; best_label = 4 * q + 3; }
           }
         }
         m.sem_label[si] = static_cast<uint16_t>(best_label);
@@ -2020,7 +2040,8 @@ void launchSelectBlocks(const DeviceMap& m, const BatchParams& p, int cull_grid,
     else { if (pb) itemCompactKernel<8, true><<<cull_grid, 256, 0, s>>>(m, p); else itemCompactKernel<8, false><<<cull_grid, 256, 0, s>>>(m, p); }
   }
 }
-static size_t fuseSmemBytes(int Lp) { return static_cast<size_t>(std::max(Lp, 2)) * kFuseThreads * sizeof(float); }
+// fuseKernel's rows; fuseKernelMlp's [Lp][kFuseThreads] rows fit in the same allocation (fuseRowStride(Lp) >= Lp)
+static size_t fuseSmemBytes(int Lp) { return static_cast<size_t>(fuseRowStride(Lp)) * kFuseThreads * sizeof(float); }
 int fuseBlocksPerSm(int vps, int Lp) {
   int n = 0;
   if (vps == 16) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fuseKernel<16, 1, false, false>, kFuseThreads, fuseSmemBytes(Lp));

@@ -38,6 +38,8 @@ struct BatchParams {
   float adaptive_thr;
   int sem_mode, L;
   float mle_diag, mle_off, mle_init;
+  uint32_t label_frames;  // bit b: frame b has a label image the semantic mode reads (object image in BINARY mode)
+  uint32_t mask_frames;   // bit b: frame b carries a dynamic mask
   unsigned long long blocked_mask;
   int lo[3], dims[3];  // union candidate block AABB of the batch (allocate mode)
   int allocate;        // 1: enumerate AABB + frustum test + insert; 0: all live slots
