@@ -163,18 +163,19 @@ __device__ __forceinline__ float measurementWeight(const BatchParams& p, float d
   return w;
 }
 
-// ProjectionInterpolator::interpolateColor (UP App. A.6 step 5; docs/ORACLE_SPEC.md §5.6): nearest -> the pixel's
-// colour; bilinear -> per channel ((w0 c0 + w1 c1) + w2 c2) + w3 c3 over the taps (u,v), (u,v+1), (u+1,v), (u+1,v+1),
-// truncated to u8.
-__device__ __forceinline__ uchar3 measuredColor(const BatchParams& p, const FrameView& f, const Taps& t) {
-  const uint8_t* __restrict__ p0 = f.color + (static_cast<size_t>(t.v) * p.W + t.u) * 3;
-  if (!t.bilinear) return make_uchar3(__ldg(p0), __ldg(p0 + 1), __ldg(p0 + 2));
+// ProjectionInterpolator::interpolateColor (UP App. A.6 step 5; docs/ORACLE_SPEC.md §5.6): nearest -> the colour of
+// pixel i; bilinear -> per channel ((w0 c0 + w1 c1) + w2 c2) + w3 c3 over the taps (u,v), (u,v+1), (u+1,v), (u+1,v+1)
+// with pixel i = (u,v), truncated to u8.
+__device__ __forceinline__ uchar3 measuredColor(const BatchParams& p, const FrameView& f, int i, bool bilinear, float w0,
+                                                float w1, float w2, float w3) {
+  const uint8_t* __restrict__ p0 = f.color + static_cast<size_t>(i) * 3;
+  if (!bilinear) return make_uchar3(__ldg(p0), __ldg(p0 + 1), __ldg(p0 + 2));
   const uint8_t* __restrict__ p1 = p0 + static_cast<size_t>(p.W) * 3;
   uint8_t o[3];
 #pragma unroll
   for (int ch = 0; ch < 3; ++ch) {
-    const float s = ((t.w0 * static_cast<float>(__ldg(p0 + ch)) + t.w1 * static_cast<float>(__ldg(p1 + ch))) +
-                     t.w2 * static_cast<float>(__ldg(p0 + 3 + ch))) + t.w3 * static_cast<float>(__ldg(p1 + 3 + ch));
+    const float s = ((w0 * static_cast<float>(__ldg(p0 + ch)) + w1 * static_cast<float>(__ldg(p1 + ch))) +
+                     w2 * static_cast<float>(__ldg(p0 + 3 + ch))) + w3 * static_cast<float>(__ldg(p1 + 3 + ch));
     o[ch] = static_cast<uint8_t>(static_cast<int>(s));
   }
   return make_uchar3(o[0], o[1], o[2]);
@@ -645,15 +646,62 @@ __global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS
       const float u = p.fx * x / z + p.cx;
       const float v = p.fy * y / z + p.cy;
       if (u < 0.f || u > static_cast<float>(p.W - 1) || v < 0.f || v > static_cast<float>(p.H - 1)) continue;
-      float range = 0.f;
-      const Taps taps = computeTaps<COMPACT>(p, f, u, v, range);
-      if (!taps.valid) continue;
+      // computeTaps restated on four depth taps loaded together at clamped addresses (on the last column / row the
+      // second column / row collapses onto the first): the nearest pixel, round(u) = floor(u) + (du >= 0.5) for u >= 0,
+      // is one of the four, so the nearest fallback selects a register instead of waiting on another load.
+      const int u0 = static_cast<int>(floorf(u)), v0 = static_cast<int>(floorf(v));
+      const float du = u - static_cast<float>(u0), dv = v - static_cast<float>(v0);
+      const int i0 = v0 * p.W + u0;
+      const int su = u0 + 1 < p.W ? 1 : 0, sv = v0 + 1 < p.H ? p.W : 0;
+      const float r0 = depthAt<COMPACT>(f, i0);
+      const float r2 = depthAt<COMPACT>(f, i0 + su);
+      const float r1 = depthAt<COMPACT>(f, i0 + sv);
+      const float r3 = depthAt<COMPACT>(f, i0 + sv + su);
+      const bool inside = su != 0 && sv != 0;
+      const bool ru = du >= 0.5f, rv = dv >= 0.5f;
+      const int ti_near = i0 + (ru ? 1 : 0) + (rv ? p.W : 0);  // du = 0 on the last column, dv = 0 on the last row
+      const float w0 = (1.f - du) * (1.f - dv);
+      const float w1 = (1.f - du) * dv;
+      const float w2 = du * (1.f - dv);
+      const float w3 = du * dv;
+      bool bilinear = false;
+      if (p.interp != KB_INTERP_NEAREST) {
+        if (inside) {
+          const bool all_valid = r0 > 0.f && r1 > 0.f && r2 > 0.f && r3 > 0.f;
+          if (p.interp == KB_INTERP_ADAPTIVE) {
+            const float mx = fmaxf(fmaxf(r0, r1), fmaxf(r2, r3));
+            const float mn = fminf(fminf(r0, r1), fminf(r2, r3));
+            bilinear = all_valid && mx - mn < p.adaptive_thr;
+          } else {
+            if (!all_valid) continue;  // bilinear: invalid
+            bilinear = true;
+          }
+        } else if (p.interp != KB_INTERP_ADAPTIVE) {
+          continue;
+        }
+      }
+      float range;
+      if (bilinear) {
+        range = ((w0 * r0 + w1 * r1) + w2 * r2) + w3 * r3;
+      } else {
+        range = ru ? (rv ? r3 : r2) : (rv ? r1 : r0);
+        if (!(range > 0.f)) continue;
+      }
       const float sdf = range - z;
       if (sdf < -p.trunc) continue;
       const bool in_band = fabsf(sdf) < p.trunc;
       uint32_t label = 0;
       if (in_band) {
-        const int ti = tapIndex(p, taps);  // interpolateID: the pixel of the dominant tap
+        // interpolateID: the pixel of the dominant tap (tapIndex: ties -> the lowest tap index), or the nearest pixel
+        int ti = ti_near;
+        if (bilinear) {
+          int best = 0;
+          float bw = w0;
+          if (w1 > bw) { best = 1; bw = w1; }
+          if (w2 > bw) { best = 2; bw = w2; }
+          if (w3 > bw) { best = 3; }
+          ti = i0 + (best >> 1) + ((best & 1) ? p.W : 0);
+        }
         if (((p.mask_frames >> b) & 1u) && __ldg(&f.mask[ti]) != 0) continue;
         if (has_label_img) {
           if (binary) {
@@ -682,7 +730,7 @@ __global__ void __launch_bounds__(kFuseThreads, COLOR ? KB_FUSE_COLOR_MIN_BLOCKS
       ++n_band;
       if constexpr (COLOR) {
         if (f.color != nullptr) {  // updateVoxel: colour is merged near the surface only
-          const uchar3 cm = measuredColor(p, f, taps);
+          const uchar3 cm = measuredColor(p, f, bilinear ? i0 : ti_near, bilinear, w0, w1, w2, w3);
           const float tot = old.y + wm;
           const float ratio = tot > 0.f ? wm / tot : 0.f;
           col.x = mergeChannel(col.x, cm.x, ratio);
@@ -1056,8 +1104,9 @@ __global__ void __launch_bounds__(kFuseThreads, KB_FUSE_MIN_BLOCKS) fuseKernelCo
 
 // ---- K1, memory-level-parallel variant (experiment, KB_FUSE_MLP=G; off by default) -------------------------------
 // fuseKernel walks an item's frames one at a time: projection -> 4 depth taps -> label/mask tap -> update, i.e. two
-// to three dependent memory round trips per frame and voxel, with ~26 resident warps per SM to hide them (ncu: issue
-// slots 54 % busy, the rest is latency). Only the last step depends on the voxel state. This variant processes the
+// dependent memory round trips per in-band frame and voxel (three, with the nearest-pixel reload it had when this variant
+// was measured), with ~26 resident warps per SM to hide them (ncu, then: issue slots 54 % busy, the rest is latency).
+// Only the last step depends on the voxel state. This variant processes the
 // frames of an item in groups of G: phase A projects the voxel into all G frames and issues their 4 x G depth taps
 // together (clamped addresses, so the loads are unconditional and the nearest-pixel fallback is a select among the
 // four taps instead of another dependent load: round(u) is floor(u) or floor(u)+1); phase B1 derives taps / sdf /
