@@ -51,6 +51,7 @@ struct kb_handle {
   uint16_t* mot_depth16 = nullptr;
   float* stg_vertex = nullptr;
   float* mot_depth = nullptr;
+  float* mot_vertex = nullptr;  // vertex map of the last motion detection, when its frame carried one
   size_t stg_pixels = 0, mot_pixels = 0;
   int stg_set = 0;
   cudaStream_t copy_stream = nullptr;
@@ -110,12 +111,25 @@ struct kb_handle {
   std::vector<int32_t> h_pixel_gidx;
   std::vector<uint8_t> h_pixel_seed;
   std::vector<float> h_depth;
-  std::vector<float> h_vertex;  // host copy of a device-resident caller vertex map (cluster bounding boxes)
+  std::vector<float> h_vertex;  // host copy of the kept vertex map (host clustering of device frames)
   MotionResult motion;
   MotionTable mt{};            // device clustering table (M2-M4)
+  bool motion_vertex = false;  // the last detection's frame carried a vertex map (kept in mot_vertex)
+  // cluster lists of the last detection (kb_get_motion_clusters), flat in cluster order
+  std::vector<int32_t> mcl_counts;  // (pixels, voxels) per cluster
+  std::vector<int32_t> mcl_pixels;  // (u, v)
+  std::vector<int64_t> mcl_voxels;  // (x, y, z)
+  std::vector<float> mcl_bbox;      // min xyz, max xyz per cluster
+  // Device-built lists cluster again in a table of their own: the detection's table is reset after use (sparse) or
+  // taken over by kb_detect_objects / kb_track_measurements before the lists are asked for.
+  MotionTable lt{};
+  MotionLists ml{};
+  int* ml_gate = nullptr;     // device 1: the list table's stages always run
+  size_t ml_clusters = 0, ml_pixels = 0, ml_voxels = 0, ml_sort_bytes = 0;
+  void* ml_sort_tmp = nullptr;
   int32_t* d_dynamic = nullptr;  // device copy of the last dynamic image (usable as KB_MASK_LAST_DETECTION)
   int* h_mscal = nullptr;      // pinned mirror of the clustering scalars
-  bool motion_stale = false;   // cluster lists of the last detection not yet built on the host
+  bool motion_stale = false;   // cluster lists of the last device detection not built yet
   MotionHostParams motion_hp{};
   bool motion_have_image = false;
   bool everfree_v2 = true;     // vectorised halo fill of the ever-free pass (default since round 2; KB_EVERFREE_V2=0 disables)
@@ -305,20 +319,16 @@ int ensureShardBuffers(kb_handle* h) {
   return KB_OK;
 }
 
-int ensureMotionBuffers(kb_handle* h, size_t pixels) {
-  if (h->mot_pixels >= pixels) return KB_OK;
-  MotionTable& t = h->mt;
-  cudaFree(h->mot_depth); cudaFree(h->stg_vertex); cudaFree(h->d_pixel_gidx); cudaFree(h->d_pixel_seed);
-  cudaFree(h->d_dynamic);
+void freeMotionTable(MotionTable& t) {
   cudaFree(t.keys); cudaFree(t.count); cudaFree(t.flags); cudaFree(t.deg); cudaFree(t.parent); cudaFree(t.pix_total);
   cudaFree(t.min_seed); cudaFree(t.cluster_id); cudaFree(t.roots); cudaFree(t.scalars); cudaFree(t.pix_slot);
-  cudaFree(h->mot_depth16);
-  KB_CUDA(h, devAlloc(&h->mot_depth16, pixels, 0));
-  KB_CUDA(h, devAlloc(&h->mot_depth, pixels, 0));
-  KB_CUDA(h, devAlloc(&h->stg_vertex, pixels * 3, 0));
-  KB_CUDA(h, devAlloc(&h->d_pixel_gidx, pixels, 0));
-  KB_CUDA(h, devAlloc(&h->d_pixel_seed, pixels, 0));
-  KB_CUDA(h, devAlloc(&h->d_dynamic, pixels, 0));
+  cudaFree(t.occupied);
+  t = MotionTable{};
+}
+
+// A clean clustering table for `pixels` pixels (gate left to the caller).
+int allocMotionTable(kb_handle* h, MotionTable& t, size_t pixels) {
+  freeMotionTable(t);
   uint32_t cap = 1024;
   while (cap < 2 * pixels) cap <<= 1;
   t.mask = cap - 1;
@@ -333,11 +343,27 @@ int ensureMotionBuffers(kb_handle* h, size_t pixels) {
   KB_CUDA(h, devAlloc(&t.min_seed, cap, 0xFF));
   KB_CUDA(h, devAlloc(&t.cluster_id, cap, 0));
   KB_CUDA(h, devAlloc(&t.roots, static_cast<size_t>(t.max_roots), 0));
-  cudaFree(t.occupied);
   KB_CUDA(h, devAlloc(&t.occupied, pixels, 0));
   KB_CUDA(h, devAlloc(&t.scalars, static_cast<size_t>(kMsCount), 0));
   KB_CUDA(h, devAlloc(&t.pix_slot, pixels, 0xFF));
-  t.gate = h->dm.counters + kCtrSeeds;
+  return KB_OK;
+}
+
+int ensureMotionBuffers(kb_handle* h, size_t pixels) {
+  if (h->mot_pixels >= pixels) return KB_OK;
+  cudaFree(h->mot_depth); cudaFree(h->mot_vertex); cudaFree(h->stg_vertex); cudaFree(h->d_pixel_gidx); cudaFree(h->d_pixel_seed);
+  cudaFree(h->d_dynamic);
+  cudaFree(h->mot_depth16);
+  KB_CUDA(h, devAlloc(&h->mot_depth16, pixels, 0));
+  KB_CUDA(h, devAlloc(&h->mot_depth, pixels, 0));
+  KB_CUDA(h, devAlloc(&h->mot_vertex, pixels * 3, 0));
+  KB_CUDA(h, devAlloc(&h->stg_vertex, pixels * 3, 0));
+  KB_CUDA(h, devAlloc(&h->d_pixel_gidx, pixels, 0));
+  KB_CUDA(h, devAlloc(&h->d_pixel_seed, pixels, 0));
+  KB_CUDA(h, devAlloc(&h->d_dynamic, pixels, 0));
+  int st = allocMotionTable(h, h->mt, pixels);
+  if (st != KB_OK) return st;
+  h->mt.gate = h->dm.counters + kCtrSeeds;
   if (!h->h_mscal) KB_CUDA(h, cudaMallocHost(reinterpret_cast<void**>(&h->h_mscal), sizeof(int) * kMsCount));
   h->mot_pixels = pixels;
   return KB_OK;
@@ -410,10 +436,10 @@ int slotHwm(kb_handle* h, int* n) {
   return KB_OK;
 }
 
-// Host M2-M4 on the per-pixel voxel keys of the last M1 launch (slow path: cluster lists on demand, separation
-// distance <= 0, caller-supplied vertex maps). A caller vertex map in device memory is copied back with the other M1
-// inputs: the bounding boxes come from the vertex map, not from the back-projected depth (:396-397).
-int buildMotionClustersOnHost(kb_handle* h, const float* vertex_world, bool vertex_on_device, int32_t* image_out) {
+// Host M2-M4 on the per-pixel voxel keys of the last M1 launch (min_separation_distance <= 0, where one voxel can belong
+// to several clusters). The bounding boxes come from the frame's vertex map when it has one (:396-397): host_vertex
+// for host frames, else the copy kept on the device.
+int buildMotionClustersOnHost(kb_handle* h, const float* host_vertex, int32_t* image_out) {
   const size_t px = static_cast<size_t>(h->cam.width) * h->cam.height;
   h->h_pixel_gidx.resize(px * 3);
   h->h_pixel_seed.resize(px);
@@ -421,16 +447,140 @@ int buildMotionClustersOnHost(kb_handle* h, const float* vertex_world, bool vert
   KB_CUDA(h, cudaMemcpyAsync(h->h_pixel_gidx.data(), h->d_pixel_gidx, sizeof(int3) * px, cudaMemcpyDeviceToHost, h->stream));
   KB_CUDA(h, cudaMemcpyAsync(h->h_pixel_seed.data(), h->d_pixel_seed, px, cudaMemcpyDeviceToHost, h->stream));
   KB_CUDA(h, cudaMemcpyAsync(h->h_depth.data(), h->mot_depth, sizeof(float) * px, cudaMemcpyDeviceToHost, h->stream));
-  if (vertex_world && vertex_on_device) {
+  if (!host_vertex && h->motion_vertex) {
     h->h_vertex.resize(px * 3);
-    KB_CUDA(h, cudaMemcpyAsync(h->h_vertex.data(), vertex_world, sizeof(float) * 3 * px, cudaMemcpyDeviceToHost, h->stream));
-    vertex_world = h->h_vertex.data();
+    KB_CUDA(h, cudaMemcpyAsync(h->h_vertex.data(), h->mot_vertex, sizeof(float) * 3 * px, cudaMemcpyDeviceToHost, h->stream));
+    host_vertex = h->h_vertex.data();
   }
   KB_CUDA(h, cudaStreamSynchronize(h->stream));
-  std::vector<int32_t> scratch;
-  if (!image_out) { scratch.assign(px, 0); image_out = scratch.data(); }
-  clusterMotion(h->motion_hp, h->h_pixel_gidx.data(), h->h_pixel_seed.data(), h->h_depth.data(), vertex_world,
+  clusterMotion(h->motion_hp, h->h_pixel_gidx.data(), h->h_pixel_seed.data(), h->h_depth.data(), host_vertex,
                 image_out, &h->motion);
+  const auto& cl = h->motion.clusters;
+  for (const MotionCluster& c : cl) {
+    h->mcl_counts.push_back(static_cast<int32_t>(c.pixels.size() / 2));
+    h->mcl_counts.push_back(static_cast<int32_t>(c.voxels.size() / 3));
+    h->mcl_pixels.insert(h->mcl_pixels.end(), c.pixels.begin(), c.pixels.end());
+    h->mcl_voxels.insert(h->mcl_voxels.end(), c.voxels.begin(), c.voxels.end());
+    h->mcl_bbox.insert(h->mcl_bbox.end(), c.bbox, c.bbox + 6);
+  }
+  return KB_OK;
+}
+
+void freeMotionLists(kb_handle* h) {
+  MotionLists& l = h->ml;
+  cudaFree(l.pix_count); cudaFree(l.vox_count); cudaFree(l.pix_off); cudaFree(l.vox_off); cudaFree(l.pix_fill);
+  cudaFree(l.vox_fill); cudaFree(l.box_min); cudaFree(l.box_max); cudaFree(l.bbox); cudaFree(l.vox_next);
+  cudaFree(l.pixels_uv); cudaFree(l.vox_keys); cudaFree(l.vox_sorted); cudaFree(l.voxels_xyz);
+  cudaFree(h->ml_gate); cudaFree(h->ml_sort_tmp);
+  freeMotionTable(h->lt);
+  l = MotionLists{};
+  h->ml_gate = nullptr;
+  h->ml_sort_tmp = nullptr;
+  h->ml_clusters = h->ml_pixels = h->ml_voxels = h->ml_sort_bytes = 0;
+}
+
+// Cluster lists of the last device detection, built on the device from what the detection kept: its M1 output
+// (d_pixel_gidx / d_pixel_seed, written only by the motion calls) and its vertex map or depth. Only the lists cross
+// to the host.
+int buildMotionListsOnDevice(kb_handle* h) {
+  const size_t px = static_cast<size_t>(h->cam.width) * h->cam.height;
+  const int K = h->h_mscal[kMsClusters];
+  MotionLists& l = h->ml;
+  MotionTable& t = h->lt;
+  if (!t.keys || t.max_roots < static_cast<int>(px)) {  // first call, or the camera grew
+    KB_CUDA(h, cudaStreamSynchronize(h->stream));
+    freeMotionLists(h);
+    int st = allocMotionTable(h, t, px);
+    if (st != KB_OK) return st;
+    const int one = 1;
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&h->ml_gate), sizeof(int)));
+    KB_CUDA(h, cudaMemcpy(h->ml_gate, &one, sizeof(int), cudaMemcpyHostToDevice));
+    t.gate = h->ml_gate;
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.vox_next), sizeof(int) * (static_cast<size_t>(t.mask) + 1)));
+  }
+  if (h->ml_clusters < static_cast<size_t>(K)) {
+    KB_CUDA(h, cudaStreamSynchronize(h->stream));
+    cudaFree(l.pix_count); cudaFree(l.vox_count); cudaFree(l.pix_off); cudaFree(l.vox_off); cudaFree(l.pix_fill);
+    cudaFree(l.vox_fill); cudaFree(l.box_min); cudaFree(l.box_max); cudaFree(l.bbox);
+    const size_t n = static_cast<size_t>(K);
+    h->ml_clusters = 0;
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.pix_count), sizeof(int) * n));
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.vox_count), sizeof(int) * n));
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.pix_off), sizeof(int) * (n + 1)));
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.vox_off), sizeof(int) * (n + 1)));
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.pix_fill), sizeof(int) * n));
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.vox_fill), sizeof(int) * n));
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.box_min), sizeof(unsigned int) * 3 * n));
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.box_max), sizeof(unsigned int) * 3 * n));
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.bbox), sizeof(float) * 6 * n));
+    h->ml_clusters = n;
+  }
+  const int P = static_cast<int>(px);
+  const int D = static_cast<int>(std::ceil(h->mot.min_separation_distance));
+  launchMotionListCounts(t, l, h->d_pixel_gidx, h->d_pixel_seed, P, h->mot.neighbor_connectivity, D, h->mot.min_cluster_size,
+                         h->mot.max_cluster_size, K, h->stream);
+  KB_CUDA(h, cudaGetLastError());
+  std::vector<int32_t> npix(K), nvox(K);
+  int scal[kMsCount];
+  KB_CUDA(h, cudaMemcpyAsync(npix.data(), l.pix_count, sizeof(int) * K, cudaMemcpyDeviceToHost, h->stream));
+  KB_CUDA(h, cudaMemcpyAsync(nvox.data(), l.vox_count, sizeof(int) * K, cudaMemcpyDeviceToHost, h->stream));
+  KB_CUDA(h, cudaMemcpyAsync(scal, t.scalars, sizeof(scal), cudaMemcpyDeviceToHost, h->stream));
+  KB_CUDA(h, cudaStreamSynchronize(h->stream));
+  if (scal[kMsClusters] != K) return fail(h, KB_ERR_STATE, "the cluster lists disagree with the detection");
+  std::vector<int32_t> off(2 * (static_cast<size_t>(K) + 1));  // pixel offsets, then voxel offsets
+  int32_t* poff = off.data();
+  int32_t* voff = off.data() + K + 1;
+  int64_t tp = 0, tv = 0;
+  for (int c = 0; c < K; ++c) {
+    poff[c] = static_cast<int32_t>(tp);
+    voff[c] = static_cast<int32_t>(tv);
+    tp += npix[c];
+    tv += nvox[c];
+    if (tp > INT32_MAX) return fail(h, KB_ERR_CAPACITY, "more than 2^31 cluster pixels");
+  }
+  poff[K] = static_cast<int32_t>(tp);
+  voff[K] = static_cast<int32_t>(tv);
+  if (h->ml_pixels < static_cast<size_t>(tp)) {
+    cudaFree(l.pixels_uv);
+    h->ml_pixels = 0;
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.pixels_uv), sizeof(int32_t) * 2 * tp));
+    h->ml_pixels = static_cast<size_t>(tp);
+  }
+  if (h->ml_voxels < static_cast<size_t>(tv)) {
+    cudaFree(l.vox_keys); cudaFree(l.vox_sorted); cudaFree(l.voxels_xyz);
+    h->ml_voxels = 0;
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.vox_keys), sizeof(unsigned long long) * tv));
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.vox_sorted), sizeof(unsigned long long) * tv));
+    KB_CUDA(h, cudaMalloc(reinterpret_cast<void**>(&l.voxels_xyz), sizeof(int64_t) * 3 * tv));
+    h->ml_voxels = static_cast<size_t>(tv);
+  }
+  KB_CUDA(h, cudaMemcpyAsync(l.pix_off, poff, sizeof(int32_t) * (K + 1), cudaMemcpyHostToDevice, h->stream));
+  KB_CUDA(h, cudaMemcpyAsync(l.vox_off, voff, sizeof(int32_t) * (K + 1), cudaMemcpyHostToDevice, h->stream));
+  MotionBoxParams b{};
+  const MotionHostParams& mp = h->motion_hp;
+  b.vertex = h->motion_vertex ? h->mot_vertex : nullptr;
+  b.depth = h->mot_depth;
+  b.W = mp.W; b.fx = mp.fx; b.fy = mp.fy; b.cx = mp.cx; b.cy = mp.cy;
+  std::memcpy(b.Rw, mp.Rw, sizeof(b.Rw));
+  std::memcpy(b.tw, mp.tw, sizeof(b.tw));
+  size_t bytes = 0;
+  KB_CUDA(h, launchMotionListFill(t, l, b, P, K, static_cast<int>(tv), nullptr, &bytes, h->stream));
+  if (h->ml_sort_bytes < bytes) {
+    cudaFree(h->ml_sort_tmp);
+    h->ml_sort_bytes = 0;
+    KB_CUDA(h, cudaMalloc(&h->ml_sort_tmp, bytes));
+    h->ml_sort_bytes = bytes;
+  }
+  KB_CUDA(h, launchMotionListFill(t, l, b, P, K, static_cast<int>(tv), h->ml_sort_tmp, &bytes, h->stream));
+  h->mcl_counts.resize(2 * static_cast<size_t>(K));
+  for (int c = 0; c < K; ++c) { h->mcl_counts[2 * c] = npix[c]; h->mcl_counts[2 * c + 1] = nvox[c]; }
+  h->mcl_pixels.resize(static_cast<size_t>(2 * tp));
+  h->mcl_voxels.resize(static_cast<size_t>(3 * tv));
+  h->mcl_bbox.resize(6 * static_cast<size_t>(K));
+  KB_CUDA(h, cudaMemcpyAsync(h->mcl_pixels.data(), l.pixels_uv, sizeof(int32_t) * 2 * tp, cudaMemcpyDeviceToHost, h->stream));
+  KB_CUDA(h, cudaMemcpyAsync(h->mcl_voxels.data(), l.voxels_xyz, sizeof(int64_t) * 3 * tv, cudaMemcpyDeviceToHost, h->stream));
+  KB_CUDA(h, cudaMemcpyAsync(h->mcl_bbox.data(), l.bbox, sizeof(float) * 6 * K, cudaMemcpyDeviceToHost, h->stream));
+  KB_CUDA(h, cudaStreamSynchronize(h->stream));
   h->motion_stale = false;
   return KB_OK;
 }
@@ -617,8 +767,9 @@ int kb_destroy(kb_handle* h) {
   cudaFree(h->stg_depth); cudaFree(h->stg_label); cudaFree(h->stg_mask); cudaFree(h->stg_object);
   cudaFree(h->stg_vertex); cudaFree(h->d_pixel_gidx); cudaFree(h->d_pixel_seed); cudaFree(h->d_removed);
   cudaFree(h->d_dynamic);
-  { MotionTable& t = h->mt; cudaFree(t.keys); cudaFree(t.count); cudaFree(t.flags); cudaFree(t.deg); cudaFree(t.parent);
-    cudaFree(t.pix_total); cudaFree(t.min_seed); cudaFree(t.cluster_id); cudaFree(t.roots); cudaFree(t.scalars); cudaFree(t.pix_slot); cudaFree(t.occupied); }
+  freeMotionTable(h->mt);
+  freeMotionLists(h);
+  cudaFree(h->mot_vertex);
   if (h->h_mscal) cudaFreeHost(h->h_mscal);
   cudaFree(h->stg_depth16); cudaFree(h->stg_label8); cudaFree(h->mot_depth16);
   cudaFree(h->mot_depth); cudaFree(h->tile_max); cudaFree(h->work_slots); cudaFree(h->work_masks); cudaFree(h->work_upd); cudaFree(h->item_fmask); cudaFree(h->item_list);
@@ -1619,7 +1770,7 @@ int kb_scan_object_confidence(kb_handle* h, float min_confidence, int32_t min_ob
 }
 
 // M1 launch shared by kb_detect_motion and kb_spin_once: stages depth / vertex map, resets the seed counter,
-// enqueues the per-pixel lookup and records the host parameters for lazily built cluster lists.
+// enqueues the per-pixel lookup and records what lazily built cluster lists need (depth, vertex map, parameters).
 static int enqueueMotionLookup(kb_handle* h, const kb_frame* f, uint8_t* shard_flags = nullptr) {
   if (h) h->main_dirty = true;  // KB_PIPELINE: the next prologue must wait for this main-stream work
   const kb_camera& c = h->cam;
@@ -1642,7 +1793,12 @@ static int enqueueMotionLookup(kb_handle* h, const kb_frame* f, uint8_t* shard_f
   } else if ((st = stage(h, f->depth, h->mot_depth, px, f->memory, &p.depth)) != KB_OK) {
     return st;
   }
-  if ((st = stage(h, f->vertex_world, h->stg_vertex, px * 3, f->memory, &p.vertex)) != KB_OK) return st;
+  h->motion_vertex = f->vertex_world != nullptr;
+  if (f->vertex_world) {  // kept for the cluster lists' boxes: a device map is only borrowed for the call
+    KB_CUDA(h, cudaMemcpyAsync(h->mot_vertex, f->vertex_world, sizeof(float) * 3 * px,
+                               f->memory == KB_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
+    p.vertex = h->mot_vertex;
+  }
   p.pixel_gidx = h->d_pixel_gidx;
   p.pixel_seed = h->d_pixel_seed;
   p.pixel_flags = shard_flags;
@@ -1663,13 +1819,15 @@ static int enqueueMotionLookup(kb_handle* h, const kb_frame* f, uint8_t* shard_f
   mp.min_separation_distance = h->mot.min_separation_distance;
   h->motion.clusters.clear();
   h->motion.n_seeds = 0;
+  h->mcl_counts.clear(); h->mcl_pixels.clear(); h->mcl_voxels.clear(); h->mcl_bbox.clear();
   h->motion_stale = false;
   h->motion_have_image = false;
   return KB_OK;
 }
 
-// M2-M4 on the device (connected components over the voxels that contain points); every stage is gated by the
-// device-side seed counter, so this can be enqueued without knowing whether M1 found seeds.
+// M2-M4 on the device (connected components over the voxels that contain points) for min_separation_distance > 0, with
+// or without a caller vertex map; every stage is gated by the device-side seed counter, so this can be enqueued without
+// knowing whether M1 found seeds. The cluster lists are built only when asked for (buildMotionListsOnDevice).
 static int enqueueDeviceClustering(kb_handle* h) {
   const size_t px = static_cast<size_t>(h->cam.width) * h->cam.height;
   const int D = static_cast<int>(std::ceil(h->mot.min_separation_distance));
@@ -1702,8 +1860,7 @@ int kb_detect_motion(kb_handle* h, const kb_frame* f, int32_t* dynamic_image_out
   if (seed_pixels == 0) {
     std::memset(dynamic_image_out, 0, sizeof(int32_t) * px);
   } else {
-    bool device_path = h->mot.min_separation_distance > 0.f && f->vertex_world == nullptr;
-    if (device_path) {
+    if (h->mot.min_separation_distance > 0.f) {
       if ((st = enqueueDeviceClustering(h)) != KB_OK) return st;
       KB_CUDA(h, cudaMemcpyAsync(dynamic_image_out, h->d_dynamic, sizeof(int32_t) * px, cudaMemcpyDeviceToHost, h->stream));
       KB_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -1713,7 +1870,8 @@ int kb_detect_motion(kb_handle* h, const kb_frame* f, int32_t* dynamic_image_out
       h->motion_have_image = true;
     } else {
       std::memset(dynamic_image_out, 0, sizeof(int32_t) * px);
-      if ((st = buildMotionClustersOnHost(h, f->vertex_world, f->memory == KB_MEM_DEVICE, dynamic_image_out)) != KB_OK) return st;
+      const float* host_vertex = f->memory == KB_MEM_DEVICE ? nullptr : f->vertex_world;
+      if ((st = buildMotionClustersOnHost(h, host_vertex, dynamic_image_out)) != KB_OK) return st;
       n_clusters_out = static_cast<int>(h->motion.clusters.size());
       KB_CUDA(h, cudaMemcpyAsync(h->d_dynamic, dynamic_image_out, sizeof(int32_t) * px, cudaMemcpyHostToDevice, h->stream));
       h->motion_have_image = true;
@@ -1731,8 +1889,8 @@ int kb_spin_once(kb_handle* h, const kb_frame* f, int32_t* dynamic_image_out, in
   KB_CUDA(h, cudaSetDevice(h->device));
   const size_t px = static_cast<size_t>(h->cam.width) * h->cam.height;
   int st;
-  if (!(h->mot.min_separation_distance > 0.f) || f->vertex_world != nullptr) {
-    // configurations the device clustering does not cover: run the three steps one after the other
+  if (!(h->mot.min_separation_distance > 0.f)) {
+    // the host clustering (one voxel may belong to several clusters): run the three steps one after the other
     std::vector<int32_t> tmp;
     int32_t* img = dynamic_image_out;
     if (!img) { tmp.assign(px, 0); img = tmp.data(); }
@@ -2271,21 +2429,15 @@ int kb_get_motion_clusters(kb_handle* h, int32_t* counts, int32_t* pixels_uv, in
   if (!h) return KB_ERR_INVALID;
   if (h->motion_stale) {
     KB_CUDA(h, cudaSetDevice(h->device));
-    const int st = buildMotionClustersOnHost(h, nullptr, false, nullptr);
+    const int st = buildMotionListsOnDevice(h);
     if (st != KB_OK) return st;
   }
-  size_t tp = 0, tv = 0;
-  const auto& cl = h->motion.clusters;
-  for (size_t c = 0; c < cl.size(); ++c) {
-    if (counts) { counts[c * 2] = static_cast<int32_t>(cl[c].pixels.size() / 2); counts[c * 2 + 1] = static_cast<int32_t>(cl[c].voxels.size() / 3); }
-    if (pixels_uv) std::memcpy(pixels_uv + tp * 2, cl[c].pixels.data(), cl[c].pixels.size() * sizeof(int32_t));
-    if (voxels_xyz) std::memcpy(voxels_xyz + tv * 3, cl[c].voxels.data(), cl[c].voxels.size() * sizeof(int64_t));
-    if (bbox_min_max) std::memcpy(bbox_min_max + c * 6, cl[c].bbox, sizeof(float) * 6);
-    tp += cl[c].pixels.size() / 2;
-    tv += cl[c].voxels.size() / 3;
-  }
-  if (total_pixels) *total_pixels = static_cast<int32_t>(tp);
-  if (total_voxels) *total_voxels = static_cast<int32_t>(tv);
+  if (counts) std::memcpy(counts, h->mcl_counts.data(), sizeof(int32_t) * h->mcl_counts.size());
+  if (pixels_uv) std::memcpy(pixels_uv, h->mcl_pixels.data(), sizeof(int32_t) * h->mcl_pixels.size());
+  if (voxels_xyz) std::memcpy(voxels_xyz, h->mcl_voxels.data(), sizeof(int64_t) * h->mcl_voxels.size());
+  if (bbox_min_max) std::memcpy(bbox_min_max, h->mcl_bbox.data(), sizeof(float) * h->mcl_bbox.size());
+  if (total_pixels) *total_pixels = static_cast<int32_t>(h->mcl_pixels.size() / 2);
+  if (total_voxels) *total_voxels = static_cast<int32_t>(h->mcl_voxels.size() / 3);
   return KB_OK;
 }
 

@@ -18,6 +18,8 @@
 
 #include <algorithm>
 
+#include <cub/device/device_segmented_sort.cuh>
+
 #include "kb_motion_device.cuh"
 #include "kb_unionfind.cuh"
 
@@ -188,7 +190,7 @@ __global__ void vtRankKernel(MotionTable t, int min_size, int max_size) {
         const unsigned long long pq = t.pix_total[q];
         if (pq >= static_cast<unsigned long long>(max(min_size, 0)) && pq <= static_cast<unsigned long long>(max(max_size, 0)) && t.min_seed[q] < mine) ++rank;
       }
-      id = min(rank + 1, 255);  // ids saturate at 255 (:390-395)
+      id = rank + 1;  // the image saturates it at 255 (:390-395); the cluster lists need the rank itself
       atomicAdd(&s_kept, 1);
     }
     t.cluster_id[r] = id;
@@ -204,7 +206,7 @@ __global__ void vtWriteImageKernel(MotionTable t, int32_t* __restrict__ image, i
   int id = 0;
   if (*t.gate != 0) {
     const int slot = t.pix_slot[px];
-    if (slot >= 0 && t.deg[slot] != 0) id = t.cluster_id[ufFind(t.parent, slot)];
+    if (slot >= 0 && t.deg[slot] != 0) id = min(t.cluster_id[ufFind(t.parent, slot)], 255);
   }
   image[px] = id;  // no seeds: an all-zero dynamic image
 }
@@ -276,7 +278,156 @@ __global__ void vtCleanupKernel(MotionTable t) {
   }
 }
 
+// ---- cluster lists (kb_get_motion_clusters) ----
+
+// Cluster index (0-based rank, not saturating) of an occupied slot, or -1 when the slot is in no kept cluster.
+__device__ __forceinline__ int listCluster(const MotionTable& t, int slot) {
+  if (slot < 0 || t.deg[slot] == 0) return -1;
+  return t.cluster_id[ufFind(t.parent, slot)] - 1;
+}
+
+// Reserves n consecutive entries of ctr[c] for each lane with c >= 0 and returns the first; lanes that share c take one
+// atomic between them (a cluster's voxels and pixels arrive in runs). Every lane of the warp must call it.
+__device__ __forceinline__ int warpReserve(int* ctr, int c, int n) {
+  const unsigned peers = __match_any_sync(0xffffffffu, c);
+  const int lane = threadIdx.x & 31;
+  int before = 0, total = 0;
+  for (int l = 0; l < 32; ++l) {
+    const int v = __shfl_sync(0xffffffffu, n, l);
+    if ((peers >> l) & 1u) {
+      total += v;
+      if (l < lane) before += v;
+    }
+  }
+  const int leader = __ffs(peers) - 1;
+  int base = 0;
+  if (lane == leader && c >= 0) base = atomicAdd(&ctr[c], total);
+  return __shfl_sync(0xffffffffu, base, leader) + before;
+}
+
+// Order-preserving integer image of a float: min / max of the images is the IEEE 754-2019 minimum / maximum, which
+// puts -0 below +0, so a box does not depend on the (unspecified) order of the cluster's pixels.
+__device__ __forceinline__ unsigned int floatOrder(float f) {
+  const unsigned int b = __float_as_uint(f);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float orderFloat(unsigned int o) {
+  return __uint_as_float((o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o);
+}
+
+// Per-cluster pixel counts (from the roots) and voxel counts. Warps walk the occupied list together (warpReserve).
+__global__ void __launch_bounds__(256) lsCountKernel(MotionTable t, MotionLists l) {
+  const int n = t.scalars[kMsOccupied];
+  const int lane = threadIdx.x & 31;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i - lane < n; i += gridDim.x * blockDim.x) {
+    const int slot = i < n ? t.occupied[i] : -1;
+    const int c = listCluster(t, slot);
+    warpReserve(l.vox_count, c, 1);
+    if (c >= 0 && t.parent[slot] == slot) l.pix_count[c] = static_cast<int>(t.pix_total[slot]);
+  }
+}
+
+// Places every kept voxel's key in its cluster's voxel range and reserves count * multiplicity pixel positions for it
+// (the reference appends an absorbed voxel's pixels once per adjacent seed).
+__global__ void __launch_bounds__(256) lsVoxelKernel(MotionTable t, MotionLists l) {
+  const int n = t.scalars[kMsOccupied];
+  const int lane = threadIdx.x & 31;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i - lane < n; i += gridDim.x * blockDim.x) {
+    const int slot = i < n ? t.occupied[i] : -1;
+    const int c = listCluster(t, slot);
+    const int mult = c < 0 ? 0 : ((t.flags[slot] & kMvSeed) ? 1 : t.deg[slot]);
+    const int v = warpReserve(l.vox_fill, c, 1);
+    const int p = warpReserve(l.pix_fill, c, c < 0 ? 0 : static_cast<int>(t.count[slot]) * mult);
+    if (c >= 0) {
+      l.vox_keys[l.vox_off[c] + v] = t.keys[slot];
+      l.vox_next[slot] = l.pix_off[c] + p;
+    }
+  }
+}
+
+// Writes each pixel of a kept voxel at its voxel's next position and at the same place in every further copy, and folds
+// its world point into the cluster's box (one atomic per run of same-cluster lanes per bound).
+__global__ void __launch_bounds__(256) lsPixelKernel(MotionTable t, MotionLists l, const __grid_constant__ MotionBoxParams b, int P) {
+  const int px = blockIdx.x * blockDim.x + threadIdx.x;
+  const int slot = px < P ? t.pix_slot[px] : -1;
+  const int c = listCluster(t, slot);
+  const int u = px % b.W, v = px / b.W;
+  float w[3] = {0.f, 0.f, 0.f};
+  if (c >= 0) {
+    const int n = static_cast<int>(t.count[slot]);
+    const int mult = (t.flags[slot] & kMvSeed) ? 1 : t.deg[slot];
+    const int pos = atomicAdd(&l.vox_next[slot], 1);
+    for (int k = 0; k < mult; ++k) {
+      l.pixels_uv[2 * (pos + k * n)] = u;
+      l.pixels_uv[2 * (pos + k * n) + 1] = v;
+    }
+    if (b.vertex) {
+      w[0] = b.vertex[3 * px]; w[1] = b.vertex[3 * px + 1]; w[2] = b.vertex[3 * px + 2];
+    } else {  // kb_motion_host.cpp's back-projection, op for op
+      const float d = b.depth[px];
+      const float x = __fmul_rn(__fdiv_rn(__fsub_rn(static_cast<float>(u), b.cx), b.fx), d);
+      const float y = __fmul_rn(__fdiv_rn(__fsub_rn(static_cast<float>(v), b.cy), b.fy), d);
+      for (int a = 0; a < 3; ++a)
+        w[a] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(b.Rw[3 * a], x), __fmul_rn(b.Rw[3 * a + 1], y)), __fmul_rn(b.Rw[3 * a + 2], d)), b.tw[a]);
+    }
+  }
+  const unsigned peers = __match_any_sync(0xffffffffu, c);
+  const bool leader = (threadIdx.x & 31) == __ffs(peers) - 1;
+  for (int a = 0; a < 3; ++a) {
+    const unsigned int o = floatOrder(w[a]);
+    const unsigned int lo = __reduce_min_sync(peers, o), hi = __reduce_max_sync(peers, o);
+    if (leader && c >= 0) {
+      atomicMin(&l.box_min[3 * c + a], lo);
+      atomicMax(&l.box_max[3 * c + a], hi);
+    }
+  }
+}
+
+__global__ void lsDecodeKernel(MotionLists l, int n_voxels, int n_clusters) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_voxels; i += gridDim.x * blockDim.x) {
+    int x, y, z;
+    keyToVox(l.vox_sorted[i], x, y, z);
+    l.voxels_xyz[3 * i] = x; l.voxels_xyz[3 * i + 1] = y; l.voxels_xyz[3 * i + 2] = z;
+  }
+  for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < n_clusters; c += gridDim.x * blockDim.x)
+    for (int a = 0; a < 3; ++a) {
+      l.bbox[6 * c + a] = orderFloat(l.box_min[3 * c + a]);
+      l.bbox[6 * c + 3 + a] = orderFloat(l.box_max[3 * c + a]);
+    }
+}
+
 }  // namespace
+
+void launchMotionListCounts(const MotionTable& t, const MotionLists& l, const int3* gidx, const uint8_t* seed, int P, int conn,
+                            int D, int min_size, int max_size, int n_clusters, cudaStream_t s) {
+  vtInitSparseKernel<<<1, 32, 0, s>>>(t);
+  vtInsertKernel<<<(P + 255) / 256, 256, 0, s>>>(t, gidx, seed, P);
+  vtLinkKernel<<<smCount() * 4, 256, 0, s>>>(t, conn);
+  if (D > 1) vtMergeNearKernel<<<smCount() * 4, 256, 0, s>>>(t, D);
+  vtReduceSparseKernel<<<smCount(), 256, 0, s>>>(t);
+  vtRankKernel<<<1, 1024, 0, s>>>(t, min_size, max_size);
+  cudaMemsetAsync(l.vox_count, 0, sizeof(int) * n_clusters, s);
+  lsCountKernel<<<smCount() * 4, 256, 0, s>>>(t, l);
+}
+
+cudaError_t launchMotionListFill(const MotionTable& t, const MotionLists& l, const MotionBoxParams& b, int P, int n_clusters,
+                                 int total_voxels, void* sort_tmp, size_t* sort_tmp_bytes, cudaStream_t s) {
+  if (!sort_tmp)  // size query only
+    return cub::DeviceSegmentedSort::SortKeys(nullptr, *sort_tmp_bytes, l.vox_keys, l.vox_sorted, total_voxels, n_clusters,
+                                              l.vox_off, l.vox_off + 1, s);
+  cudaMemsetAsync(l.pix_fill, 0, sizeof(int) * n_clusters, s);
+  cudaMemsetAsync(l.vox_fill, 0, sizeof(int) * n_clusters, s);
+  cudaMemsetAsync(l.box_min, 0xFF, sizeof(unsigned int) * 3 * n_clusters, s);
+  cudaMemsetAsync(l.box_max, 0, sizeof(unsigned int) * 3 * n_clusters, s);
+  lsVoxelKernel<<<smCount() * 4, 256, 0, s>>>(t, l);
+  lsPixelKernel<<<(P + 255) / 256, 256, 0, s>>>(t, l, b, P);
+  const cudaError_t e = cub::DeviceSegmentedSort::SortKeys(sort_tmp, *sort_tmp_bytes, l.vox_keys, l.vox_sorted, total_voxels,
+                                                           n_clusters, l.vox_off, l.vox_off + 1, s);
+  if (e != cudaSuccess) return e;
+  lsDecodeKernel<<<smCount(), 256, 0, s>>>(l, total_voxels, n_clusters);
+  vtCleanupKernel<<<smCount(), 256, 0, s>>>(t);  // the list table stays clean for the next call
+  return cudaGetLastError();
+}
 
 void launchMotionClusteringSparse(const MotionTable& t, const int3* gidx, const uint8_t* seed, int P, int conn, int D,
                                   int min_size, int max_size, int32_t* image, bool table_dirty, cudaStream_t s) {
