@@ -371,12 +371,15 @@ typedef struct kb_object_detector_config {
  * of the ObjectIntegrator, object_integrator.cpp:76-79). The frame needs depth (+ pose, or vertex_world) and label.
  * Cluster ids: 2D mode exactly as the reference (creation order of the column-major scan, ids of filtered clusters
  * are not reused); 3D mode: semantic ids ascending (std::map, connected_semantics.h:88), clusters of one id ordered
- * by their smallest voxel in (z, y, x) order — a determinisation of the reference's unordered_map iteration. */
+ * by their smallest voxel in (z, y, x) order — a determinisation of the reference's unordered_map iteration. 3D mode
+ * skips pixels whose vertex has a non-finite coordinate or whose voxel lies outside +-2^17 cells (docs/ORACLE_SPEC.md
+ * §10); the size filter runs before the ranking, and KB_ERR_CAPACITY means more than 4096 clusters passed it. */
 int kb_detect_objects(kb_handle* h, const kb_object_detector_config* config, const kb_frame* frame,
                       int32_t* object_image_out, int32_t* n_clusters);
 /* Clusters of the last kb_detect_objects call (MeasurementCluster id / semantics.category_id / pixels,
  * measurement_clusters.h:63-81), ascending id: id_semantic_count[c*3+0..2] = id, semantic id, #pixels; then the
- * flat (u, v) pixel list in cluster order (order within a cluster unspecified). NULL pointers are skipped. */
+ * flat (u, v) pixel list in cluster order (order within a cluster unspecified). NULL pointers are skipped. Unaffected by
+ * kb_forward_instances and kb_set_camera: (u, v) are pixels of the image that was detected. */
 int kb_get_object_clusters(kb_handle* h, int32_t* id_semantic_count, int32_t* pixels_uv, int32_t* n_clusters,
                            int32_t* total_pixels);
 
@@ -402,8 +405,10 @@ int kb_forward_instances(kb_handle* h, const kb_instance_forwarding_config* conf
                          const uint8_t* id_is_background, int32_t n_background, int32_t* object_image_out,
                          int32_t* n_clusters);
 /* Clusters of the last kb_forward_instances: id_count[c*2+0..1] = id, #pixels; bbox_min_max[c*6..] = world AABB (min xyz,
- * max xyz); pixels_uv = flat (u, v) lists in cluster order, pixels within a cluster in the reference's column-major scan
- * order (u outer, v inner). NULL pointers are skipped. */
+ * max xyz; per axis the minimum / maximum over the non-NaN coordinates with -0 < +0, NaN if there is none); pixels_uv = flat
+ * (u, v) lists in cluster order, pixels within a cluster in the reference's column-major scan order (u outer, v inner);
+ * pixels_uv needs total_pixels entries, id_count / bbox_min_max n_clusters. NULL pointers are skipped. Unaffected by
+ * kb_detect_objects and kb_set_camera. */
 int kb_get_instance_clusters(kb_handle* h, int32_t* id_count, float* bbox_min_max, int32_t* pixels_uv, int32_t* n_clusters,
                              int32_t* total_pixels);
 

@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <limits>
 #include <string>
 #include <thread>
 #include <type_traits>
@@ -144,6 +145,7 @@ struct kb_handle {
   int* h_oscal = nullptr;       // pinned mirror of the clustering scalars
   size_t obj_pixels = 0;
   std::vector<int32_t> obj_image_host, obj_label_host;
+  int obj_width = 0;            // camera width of the last result (the getter decodes pixel indices with it)
   bool obj_have = false;
   // track measurements (kb_track_measurements): staged id image, per-id accumulators, packed track voxels, results
   int32_t* trk_ids = nullptr;
@@ -180,6 +182,8 @@ struct kb_handle {
   struct InstCluster { int id, count; float bbox[6]; };
   std::vector<InstCluster> inst_clusters;
   std::vector<uint8_t> inst_keep_host;
+  std::vector<int32_t> inst_label_host;  // this detector's own copy: kb_detect_objects keeps obj_label_host
+  int inst_width = 0, inst_height = 0;   // camera of the last result
   bool inst_have = false;
   // marching cubes (kb_generate_mesh): device results of the last call + host copies of the block list
   int* mesh_slots = nullptr;
@@ -1939,6 +1943,7 @@ int kb_detect_objects(kb_handle* h, const kb_object_detector_config* cfg, const 
     KB_CUDA(h, cudaMemsetAsync(h->d_object, 0, sizeof(int32_t) * px, h->stream));
     h->obj_image_host.assign(px, 0);
     h->obj_label_host.assign(px, 0);
+    h->obj_width = c.width;
     h->obj_have = true;
     if (n_clusters) *n_clusters = 0;
     return KB_OK;
@@ -1986,9 +1991,10 @@ int kb_detect_objects(kb_handle* h, const kb_object_detector_config* cfg, const 
   KB_CUDA(h, cudaMemcpyAsync(h->h_oscal, h->mt.scalars, sizeof(int) * kMsCount, cudaMemcpyDeviceToHost, h->stream));
   KB_CUDA(h, cudaMemcpyAsync(object_image_out, h->d_object, sizeof(int32_t) * px, cudaMemcpyDeviceToHost, h->stream));
   KB_CUDA(h, cudaStreamSynchronize(h->stream));
-  if (cfg->use_3d && h->h_oscal[kMsRoots] > ot.max_roots)
+  if (cfg->use_3d && h->h_oscal[kMsRoots] > ot.max_roots)  // kept clusters: the size filter runs before the ranking
     return fail(h, KB_ERR_CAPACITY, "too many semantic clusters for the device ranking");
   h->obj_image_host.assign(object_image_out, object_image_out + px);
+  h->obj_width = c.width;
   h->obj_have = true;
   if (n_clusters) *n_clusters = h->h_oscal[kMsClusters];
   return KB_OK;
@@ -2006,8 +2012,10 @@ int kb_forward_instances(kb_handle* h, const kb_instance_forwarding_config* cfg,
   if ((st = ensureObjectBuffers(h, px)) != KB_OK) return st;
   h->inst_have = false;
   h->inst_clusters.clear();
-  h->obj_label_host.assign(px, 0);
+  h->inst_label_host.assign(px, 0);
   h->inst_keep_host.assign(px, 0);
+  h->inst_width = c.width;
+  h->inst_height = c.height;
   if (!f->label && !f->label_u8) {
     std::memset(object_image_out, 0, sizeof(int32_t) * px);
     h->inst_have = true;
@@ -2044,13 +2052,13 @@ int kb_forward_instances(kb_handle* h, const kb_instance_forwarding_config* cfg,
     std::vector<uint8_t> tmp(px);
     if (f->memory == KB_MEM_DEVICE) KB_CUDA(h, cudaMemcpy(tmp.data(), f->label_u8, px, cudaMemcpyDeviceToHost));
     else std::memcpy(tmp.data(), f->label_u8, px);
-    for (size_t i = 0; i < px; ++i) h->obj_label_host[i] = tmp[i];
-    KB_CUDA(h, cudaMemcpyAsync(h->obj_label, h->obj_label_host.data(), sizeof(int) * px, cudaMemcpyHostToDevice, h->stream));
+    for (size_t i = 0; i < px; ++i) h->inst_label_host[i] = tmp[i];
+    KB_CUDA(h, cudaMemcpyAsync(h->obj_label, h->inst_label_host.data(), sizeof(int) * px, cudaMemcpyHostToDevice, h->stream));
     p.label = h->obj_label;
   } else {
     if ((st = stage(h, f->label, h->obj_label, px, f->memory, &p.label)) != KB_OK) return st;
-    if (f->memory == KB_MEM_DEVICE) KB_CUDA(h, cudaMemcpyAsync(h->obj_label_host.data(), f->label, sizeof(int) * px, cudaMemcpyDeviceToHost, h->stream));
-    else std::memcpy(h->obj_label_host.data(), f->label, sizeof(int) * px);
+    if (f->memory == KB_MEM_DEVICE) KB_CUDA(h, cudaMemcpyAsync(h->inst_label_host.data(), f->label, sizeof(int) * px, cudaMemcpyDeviceToHost, h->stream));
+    else std::memcpy(h->inst_label_host.data(), f->label, sizeof(int) * px);
   }
   if ((st = stage(h, f->vertex_world, h->stg_vertex, px * 3, f->memory, &p.vertex)) != KB_OK) return st;
   const uint8_t* bg = nullptr;
@@ -2072,9 +2080,10 @@ int kb_forward_instances(kb_handle* h, const kb_instance_forwarding_config* cfg,
   KB_CUDA(h, cudaMemcpyAsync(&bad, h->inst_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   KB_CUDA(h, cudaStreamSynchronize(h->stream));
   if (bad) return fail(h, KB_ERR_INVALID, "instance id outside 0 .. KB_MAX_INSTANCE_IDS - 1");
-  std::memcpy(object_image_out, h->obj_label_host.data(), sizeof(int32_t) * px);  // object_image = label image (:83)
+  std::memcpy(object_image_out, h->inst_label_host.data(), sizeof(int32_t) * px);  // object_image = label image (:83)
   const bool filter_by_volume = cfg->min_object_volume > 0.0 || cfg->max_object_volume > 0.0;  // :68
-  auto decode = [](unsigned int o) {
+  auto decode = [](unsigned int o, unsigned int none) {
+    if (o == none) return std::numeric_limits<float>::quiet_NaN();  // every coordinate on the axis was NaN
     const unsigned int b = (o & 0x80000000u) ? (o & 0x7FFFFFFFu) : ~o;
     float v;
     std::memcpy(&v, &b, 4);
@@ -2087,7 +2096,7 @@ int kb_forward_instances(kb_handle* h, const kb_instance_forwarding_config* cfg,
     kb_handle::InstCluster cl{};
     cl.id = id;
     cl.count = n;
-    for (int k = 0; k < 6; ++k) cl.bbox[k] = decode(bbox[static_cast<size_t>(id) * 6 + k]);
+    for (int k = 0; k < 6; ++k) cl.bbox[k] = decode(bbox[static_cast<size_t>(id) * 6 + k], k < 3 ? 0xFFFFFFFFu : 0u);
     if (filter_by_volume) {  // :128-135, BoundingBox::volume() = product of the float dimensions
       const float volume = (cl.bbox[3] - cl.bbox[0]) * (cl.bbox[4] - cl.bbox[1]) * (cl.bbox[5] - cl.bbox[2]);
       if (volume < cfg->min_object_volume || (cfg->max_object_volume > 0.0 && volume > cfg->max_object_volume)) continue;
@@ -2103,7 +2112,7 @@ int kb_get_instance_clusters(kb_handle* h, int32_t* id_count, float* bbox_min_ma
                              int32_t* total_pixels) {
   if (!h) return KB_ERR_INVALID;
   if (!h->inst_have) return fail(h, KB_ERR_STATE, "kb_forward_instances has not been called");
-  const int W = h->cam.width, H = h->cam.height;
+  const int W = h->inst_width, H = h->inst_height;
   int32_t total = 0;
   std::vector<int> base(KB_MAX_INSTANCE_IDS, -1);
   for (size_t c = 0; c < h->inst_clusters.size(); ++c) {
@@ -2119,7 +2128,7 @@ int kb_get_instance_clusters(kb_handle* h, int32_t* id_count, float* bbox_min_ma
       for (int v = 0; v < H; ++v) {
         const size_t px = static_cast<size_t>(v) * W + u;
         if (!h->inst_keep_host[px]) continue;
-        const int id = h->obj_label_host[px];
+        const int id = h->inst_label_host[px];
         if (id <= 0 || id >= KB_MAX_INSTANCE_IDS || base[id] < 0) continue;
         const int k = base[id] + fill[id]++;
         pixels_uv[2 * k] = u;
@@ -2137,7 +2146,7 @@ int kb_get_object_clusters(kb_handle* h, int32_t* id_semantic_count, int32_t* pi
   if (!h->obj_have) return fail(h, KB_ERR_STATE, "no object detection result");
   // Cluster lists are derived on demand from the object image: ascending id, semantic id = the label under any of
   // the cluster's pixels (all agree), pixels in row-major order.
-  const int W = h->cam.width;
+  const int W = h->obj_width;
   const size_t px = h->obj_image_host.size();
   std::vector<std::pair<int32_t, int32_t>> by_id;  // (id, pixel)
   by_id.reserve(px / 8);

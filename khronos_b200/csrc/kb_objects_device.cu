@@ -7,10 +7,10 @@
 //     pixels by (semantic id, voxel of the world-frame vertex at grid_size) and region-grows over the 6/26
 //     neighbourhood per semantic id. Here: every candidate pixel inserts its (id, voxel) key into an open-addressed
 //     table (O1), one warp per occupied entry probes its neighbourhood and unions through a lock-free union-find (O2),
-//     per-root atomics accumulate pixel counts and the smallest key (O3), one CTA filters by size and ranks the kept
-//     roots by smallest key — semantic id ascending like the reference's std::map, then smallest voxel in (z,y,x)
-//     order (the determinisation of the unordered_map iteration, docs/ORACLE_SPEC.md §13) — into ids 1..N (O4), and
-//     every pixel reads its root's id (O5).
+//     per-root atomics accumulate pixel counts and the smallest key (O3), the roots that pass the size filter are
+//     listed (O3b), one CTA ranks them by smallest key — semantic id ascending like the reference's std::map, then
+//     smallest voxel in (z,y,x) order (the determinisation of the unordered_map iteration, docs/ORACLE_SPEC.md §10) —
+//     into ids 1..N (O4), and every pixel reads its root's id (O5).
 //   2D mode (semanticClustering2D :148-163 + growCluster2D :165-198 + filterClusters :200-217): union-find over the
 //     pixels in the reference's column-major scan order (index u*H + v, smaller index wins, so a component's root IS
 //     its first pixel in scan order); ids = 1 + number of roots before it (prefix sum), small clusters are zeroed
@@ -47,6 +47,10 @@ __device__ __forceinline__ void objKeyDecode(unsigned long long k, int& label, i
 }
 
 __device__ __forceinline__ bool coordOk(int c) { return c >= -kCoordBias && c < kCoordBias; }
+// The same bound on a floored float coordinate; false for NaN and +-inf.
+__device__ __forceinline__ bool cellOk(float c) {
+  return c >= -static_cast<float>(kCoordBias) && c < static_cast<float>(kCoordBias);
+}
 
 __device__ __forceinline__ int osLookup(const MotionTable& t, unsigned long long key) {
   uint32_t h = static_cast<uint32_t>(mix64(key)) & t.mask;
@@ -75,7 +79,8 @@ __global__ void osInitKernel(MotionTable t) {
   t.cluster_id[slot] = 0;
 }
 
-// O1: computeCandidateVoxels. No depth-validity test, like the reference (:127-145).
+// O1: computeCandidateVoxels. No depth-validity test, like the reference (:127-145); a pixel whose vertex has a
+// non-finite coordinate, or whose voxel lies outside +-2^17 cells, is not a candidate (ORACLE_SPEC §10).
 __global__ void osInsertKernel(MotionTable t, const __grid_constant__ ObjectParams p) {
   const int px = blockIdx.x * blockDim.x + threadIdx.x;
   if (px >= p.W * p.H) return;
@@ -94,10 +99,9 @@ __global__ void osInsertKernel(MotionTable t, const __grid_constant__ ObjectPara
       wy = ((p.Rw[3] * cxn + p.Rw[4] * cyn) + p.Rw[5] * range) + p.tw[1];
       wz = ((p.Rw[6] * cxn + p.Rw[7] * cyn) + p.Rw[8] * range) + p.tw[2];
     }
-    const int gx = static_cast<int>(floorf(wx * p.inv_grid)), gy = static_cast<int>(floorf(wy * p.inv_grid)),
-              gz = static_cast<int>(floorf(wz * p.inv_grid));
-    if (coordOk(gx) && coordOk(gy) && coordOk(gz)) {
-      const unsigned long long key = objKey(label, gx, gy, gz);
+    const float fx = floorf(wx * p.inv_grid), fy = floorf(wy * p.inv_grid), fz = floorf(wz * p.inv_grid);
+    if (cellOk(fx) && cellOk(fy) && cellOk(fz)) {
+      const unsigned long long key = objKey(label, static_cast<int>(fx), static_cast<int>(fy), static_cast<int>(fz));
       uint32_t h = static_cast<uint32_t>(mix64(key)) & t.mask;
       for (uint32_t probe = 0; probe <= t.mask; ++probe) {
         unsigned long long k = t.keys[h];
@@ -137,7 +141,7 @@ __global__ void __launch_bounds__(256) osLinkKernel(MotionTable t, int full) {
   }
 }
 
-// O3: per-component pixel count, smallest key, list of roots.
+// O3: per-component pixel count and smallest key.
 __global__ void osReduceKernel(MotionTable t) {
   const int slot = blockIdx.x * blockDim.x + threadIdx.x;
   if (slot > static_cast<int>(t.mask)) return;
@@ -146,38 +150,31 @@ __global__ void osReduceKernel(MotionTable t) {
   const int root = ufFind(t.parent, slot);
   atomicAdd(&t.pix_total[root], static_cast<unsigned long long>(t.count[slot]));
   atomicMin(&t.min_seed[root], key);
-  if (root == slot) {
-    const int i = atomicAdd(&t.scalars[kMsRoots], 1);
-    if (i < t.max_roots) t.roots[i] = slot;
-  }
 }
 
-// O4: size filter (:107-111) and ids = 1 + rank of the smallest key among the kept clusters (:112). Single CTA.
-__global__ void osRankKernel(MotionTable t, int min_size, int max_size) {
+// O3b: size filter (:107-111). Only the kept roots are listed, so the ranking's capacity bounds the clusters that get
+// an id, not the specks the filter drops. kMsRoots counts every kept root, also those beyond max_roots.
+__global__ void osKeepKernel(MotionTable t, int min_size, int max_size) {
+  const int slot = blockIdx.x * blockDim.x + threadIdx.x;
+  if (slot > static_cast<int>(t.mask) || t.keys[slot] == kOsEmpty || t.parent[slot] != slot) return;
+  const unsigned long long px = t.pix_total[slot];
+  if (px < static_cast<unsigned long long>(max(min_size, 0)) || (max_size > 0 && px > static_cast<unsigned long long>(max_size)))
+    return;
+  const int i = atomicAdd(&t.scalars[kMsRoots], 1);
+  if (i < t.max_roots) t.roots[i] = slot;
+}
+
+// O4: ids = 1 + rank of the smallest key among the kept clusters (:112). Single CTA.
+__global__ void osRankKernel(MotionTable t) {
   const int n = min(t.scalars[kMsRoots], t.max_roots);
-  __shared__ int s_kept;
-  if (threadIdx.x == 0) s_kept = 0;
-  __syncthreads();
-  const unsigned long long lo = static_cast<unsigned long long>(max(min_size, 0));
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const int r = t.roots[i];
-    const unsigned long long px = t.pix_total[r];
-    int id = 0;
-    if (px >= lo && (max_size <= 0 || px <= static_cast<unsigned long long>(max_size))) {
-      const unsigned long long mine = t.min_seed[r];
-      int rank = 0;
-      for (int j = 0; j < n; ++j) {
-        const int q = t.roots[j];
-        const unsigned long long pq = t.pix_total[q];
-        if (pq >= lo && (max_size <= 0 || pq <= static_cast<unsigned long long>(max_size)) && t.min_seed[q] < mine) ++rank;
-      }
-      id = rank + 1;
-      atomicAdd(&s_kept, 1);
-    }
-    t.cluster_id[r] = id;
+    const unsigned long long mine = t.min_seed[r];
+    int rank = 0;
+    for (int j = 0; j < n; ++j) rank += t.min_seed[t.roots[j]] < mine;
+    t.cluster_id[r] = rank + 1;
   }
-  __syncthreads();
-  if (threadIdx.x == 0) t.scalars[kMsClusters] = s_kept;
+  if (threadIdx.x == 0) t.scalars[kMsClusters] = n;
 }
 
 // O5: object_image (:114-116).
@@ -313,6 +310,8 @@ __global__ void o2WriteKernel(MotionTable t, const __grid_constant__ ObjectParam
 // The detector that forwards instance ids of an upstream segmenter: per pixel a range / background test, per id a pixel
 // count and the world-frame bounding box of its vertices (for the volume filter). One pass over the image with per-id
 // atomics (ids < kMaxInstanceIds); floats are ordered through the usual sign-flip encoding so atomicMin / atomicMax apply.
+// Min / max of the encodings is the IEEE 754-2019 minimum / maximum (-0 below +0); NaN coordinates are left out, so an
+// axis stays at its initial encodings (decoded as NaN by the host) only if every coordinate on it is NaN.
 __device__ __forceinline__ unsigned int orderedBits(float f) {
   const unsigned int b = __float_as_uint(f);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
@@ -344,8 +343,10 @@ __global__ void instanceForwardKernel(const __grid_constant__ ObjectParams p, co
         }
         atomicAdd(&counts[id], 1);
         unsigned int* b = bbox + static_cast<size_t>(id) * 6;
-        atomicMin(&b[0], orderedBits(wx)); atomicMin(&b[1], orderedBits(wy)); atomicMin(&b[2], orderedBits(wz));
-        atomicMax(&b[3], orderedBits(wx)); atomicMax(&b[4], orderedBits(wy)); atomicMax(&b[5], orderedBits(wz));
+        const float w[3] = {wx, wy, wz};
+#pragma unroll
+        for (int a = 0; a < 3; ++a)
+          if (!isnan(w[a])) { atomicMin(&b[a], orderedBits(w[a])); atomicMax(&b[3 + a], orderedBits(w[a])); }
         k = 1;
       }
     }
@@ -370,7 +371,8 @@ void launchObjectClustering3D(const MotionTable& t, const ObjectParams& p, cudaS
   osInsertKernel<<<(P + 255) / 256, 256, 0, s>>>(t, p);
   osLinkKernel<<<smCount() * 4, 256, 0, s>>>(t, p.full);
   osReduceKernel<<<(cap + 255) / 256, 256, 0, s>>>(t);
-  osRankKernel<<<1, 1024, 0, s>>>(t, p.min_size, p.max_size);
+  osKeepKernel<<<(cap + 255) / 256, 256, 0, s>>>(t, p.min_size, p.max_size);
+  osRankKernel<<<1, 1024, 0, s>>>(t);
   osWriteKernel<<<(P + 255) / 256, 256, 0, s>>>(t, p.image, P);
 }
 

@@ -938,7 +938,9 @@ void Oracle::detectObjects(const kb_object_detector_config& cfg, const kb_frame&
   auto isObject = [&](int id) { return id >= 0 && id < KB_MAX_LABELS && cfg.is_object[id] != 0; };
   if (cfg.use_3d) {
     // computeCandidateVoxels (:124-146): pixels of object classes within max_range, grouped by semantic id and by
-    // the voxel (grid_size) of their world-frame vertex. NOTE: like the reference, no depth-validity test here.
+    // the voxel (grid_size) of their world-frame vertex. NOTE: like the reference, no depth-validity test here; a
+    // vertex with a non-finite coordinate or a voxel outside +-2^17 cells makes no candidate (ORACLE_SPEC §10), where
+    // the reference's float-to-integer conversion is undefined.
     float R[9], t[3], Rw[9], tw[3];
     invertPose(f.world_T_sensor, R, t, Rw, tw);
     const float inv = 1.f / cfg.grid_size;  // semanticClustering3D(data, config.grid_size) -> 1.f / grid_size (:76)
@@ -960,8 +962,12 @@ void Oracle::detectObjects(const kb_object_detector_config& cfg, const kb_frame&
                                (static_cast<float>(v) - cam_.cy) / cam_.fy * range, range};
           transform(Rw, tw, pC, p);
         }
-        const GIdx g{static_cast<int64_t>(std::floor(p[0] * inv)), static_cast<int64_t>(std::floor(p[1] * inv)),
-                     static_cast<int64_t>(std::floor(p[2] * inv))};  // spatial_hash::indexFromPoint (:142-143)
+        const float c[3] = {std::floor(p[0] * inv), std::floor(p[1] * inv), std::floor(p[2] * inv)};
+        constexpr float kCellLimit = 131072.f;  // 2^17
+        bool inside = true;
+        for (float x : c) inside = inside && x >= -kCellLimit && x < kCellLimit;  // false for NaN and +-inf
+        if (!inside) continue;
+        const GIdx g{static_cast<int64_t>(c[0]), static_cast<int64_t>(c[1]), static_cast<int64_t>(c[2])};  // spatial_hash::indexFromPoint (:142-143)
         maps[semantic_id][g].push_back({u, v});
       }
     const auto offs = neighborOffsets(cfg.use_full_connectivity ? 26 : 6);  // :58

@@ -7,6 +7,7 @@
 // behaviour is docs/ORACLE_SPEC.md §13.
 #include <algorithm>
 #include <cmath>
+#include <limits>
 
 #include "oracle.hpp"
 #include "oracle_mc_tables.hpp"
@@ -130,12 +131,17 @@ void Oracle::forwardInstances(const kb_instance_forwarding_config& cfg, const kb
     InstanceCluster cl;
     cl.id = kv.first;
     cl.pixels = kv.second;
-    for (int a = 0; a < 3; ++a) { cl.bbox[a] = 3.4e38f; cl.bbox[3 + a] = -3.4e38f; }
+    // Per axis the IEEE 754-2019 minimum / maximum over the non-NaN coordinates (-0 below +0), so the box does not
+    // depend on the pixel order; an axis without a non-NaN coordinate is NaN at both ends.
+    for (int a = 0; a < 3; ++a) cl.bbox[a] = cl.bbox[3 + a] = std::numeric_limits<float>::quiet_NaN();
     for (const Pixel& p : cl.pixels)
       for (int a = 0; a < 3; ++a) {
         const float x = vm[(static_cast<size_t>(p.v) * W + p.u) * 3 + a];
-        cl.bbox[a] = std::min(cl.bbox[a], x);
-        cl.bbox[3 + a] = std::max(cl.bbox[3 + a], x);
+        if (std::isnan(x)) continue;
+        float& lo = cl.bbox[a];
+        float& hi = cl.bbox[3 + a];
+        if (std::isnan(lo) || x < lo || (x == lo && std::signbit(x))) lo = x;
+        if (std::isnan(hi) || x > hi || (x == hi && !std::signbit(x))) hi = x;
       }
     if (filter_by_volume) {  // :128-135
       const float volume = (cl.bbox[3] - cl.bbox[0]) * (cl.bbox[4] - cl.bbox[1]) * (cl.bbox[5] - cl.bbox[2]);
